@@ -1,12 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- attention TFLOPS/s (fwd+bwd, and fwd) at seq=262144, H=32, d=128, bf16,
-bs=1 on N B200s (BASELINE.json metric), strong scaling: the global sequence is
-fixed and sharded over the N ranks (contiguous shards, non-causal -- the C2/C3
-configurations; N=1 is the local kernel with no ring).
+"""bench.py -- attention TFLOPS/s (fwd+bwd, and fwd) at H=32, d=128, bf16, bs=1 on N H100s
+(BASELINE.json metric), strong scaling: the global sequence is fixed and sharded over the N
+ranks (contiguous shards, non-causal).  Default sequence: 262144 on N > 1 GPUs (C3), 65536 on
+one GPU (C2: the local kernel with no ring; at 262144 one H100 needs about 12 s per step).
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun)
   python bench.py --impl reference ...                     CPU arm: the oracle port of the
                                                            reference's path on the host cores
+  python bench.py ... --dump-outputs DIR                   also write O, dQ, dK, dV of the last timed step
+                                                           (a seeded sample, fp32 .npy) to DIR
 
 One "step" = one forward + one backward of burst_attn_func on synthetic
 N(0,1) bf16 inputs already resident in HBM (`value`), and the same through the
@@ -31,7 +33,9 @@ import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
 H, D, B = 32, 128, 1
-METRIC = "attention fwd+bwd TFLOPS/s (bs=1, H=32, d=128, bf16; seq in config, default 262144), aggregate over GPUs"
+METRIC = ("attention fwd+bwd TFLOPS/s (bs=1, H=32, d=128, bf16; seq in config, default 262144 on N > 1 GPUs, "
+          "65536 on one), aggregate over GPUs")
+SEQ_MULTI, SEQ_SINGLE = 262144, 65536  # BASELINE.json C3 / C2
 
 
 def flops(S, mode, batch=None):
@@ -45,7 +49,8 @@ def peaks():
         p = json.load(open(path))
         return dict(burst=p["bf16_tflops"], sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                     hbm=p["hbm_gbs"], source="MEASURED_PEAKS.json")
-    return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): dense BF16 989 TFLOP/s, HBM3 3.35 TB/s; not a measured rate
+    return dict(burst=989.0, sustained=989.0, hbm=3350.0, source="H100 SXM data sheet")
 
 
 # --------------------------------------------------------------------------- #
@@ -99,7 +104,7 @@ class ClockSampler:
 
 # --------------------------------------------------------------------------- #
 def _ref_shim():
-    """baseline/ref_shim.py: the UNMODIFIED reference from the git-ignored baseline/_ref (None if that install did
+    """baseline/ref_shim.py: the UNMODIFIED reference from the git-ignored oracle/_ref (None if that install did
     not travel to this box)."""
     sys.path.insert(0, os.path.join(ROOT, "baseline"))
     try:
@@ -108,7 +113,7 @@ def _ref_shim():
             ref_shim.load()
             return ref_shim
     except Exception as e:  # noqa: BLE001
-        sys.stderr.write(f"bench.py: reference in baseline/_ref not usable ({e!r}); CPU arm falls back to the oracle port\n")
+        sys.stderr.write(f"bench.py: reference in oracle/_ref not usable ({e!r}); CPU arm falls back to the oracle port\n")
     return None
 
 
@@ -123,7 +128,7 @@ def cpu_ref_step(shim, S, Hc, Dc, dtype, W, threads):
 
 
 def cpu_port_step(S, threads, Hc=8, Dc=D):
-    """Fallback when baseline/_ref is absent: the oracle's restatement of the same path (4 simulated ring
+    """Fallback when oracle/_ref is absent: the oracle's restatement of the same path (4 simulated ring
     rounds, fp32).  Returns (s_fwd+bwd, flops_fwd+bwd)."""
     from oracle import attention_oracle as orc
     torch.set_num_threads(threads)
@@ -167,7 +172,7 @@ def cpu_baseline():
         dt, fl = cpu_port_step(4096, threads, 8, 64)
         return {"value": fl / dt / 1e12, "unit": "TFLOPS/s", "cores": threads, "kind": "port",
                 "sample": f"oracle port (torch CPU fp32) of the reference path, C1: fwd+bwd bs=1 S=4096 H=8 d=64, "
-                          f"4 simulated ring rounds, {dt:.1f} s (baseline/_ref absent on this box)"}
+                          f"4 simulated ring rounds, {dt:.1f} s (oracle/_ref absent on this box)"}
     S, Hc, Dc = 4096, 8, 64
     detail = {}
     t_all = time.time()
@@ -183,7 +188,7 @@ def cpu_baseline():
     main = detail["fp32_W4"]
     return {"value": main["fwd_bwd_gflops"] / 1e3, "unit": "TFLOPS/s", "cores": threads,
             "host_threads_available": os.cpu_count(), "kind": "reference",
-            "sample": "reference inter_normal_attn/_backward (burst_utils.py:42-100, unmodified, from baseline/_ref) on the "
+            "sample": "reference inter_normal_attn/_backward (burst_utils.py:42-100, unmodified, from oracle/_ref) on the "
                       f"host cores, C1: bs=1 S=4096 H=8 d=64, fwd+bwd; value = fp32, 4 simulated ring ranks; 1 warm-up + "
                       f"3 reps per cell, {time.time() - t_all:.1f} s in total",
             "detail_gflops": detail}
@@ -208,7 +213,7 @@ def run_reference_arm(args):
             tf, tb, fl1 = cpu_ref_step(shim, S, Hc, D, torch.bfloat16, 4, threads)
             t += tf + tb
         fl, kind, dt_name = 3.5 * fl1, "reference", "bf16"
-        what = ("reference inter_normal_attn/_backward (burst_utils.py:42-100, unmodified, baseline/_ref), torch CPU bf16, "
+        what = ("reference inter_normal_attn/_backward (burst_utils.py:42-100, unmodified, oracle/_ref), torch CPU bf16, "
                 f"{threads} threads")
     else:
         for _ in range(warm):
@@ -217,7 +222,7 @@ def run_reference_arm(args):
             dt, fl = cpu_port_step(S, threads)
             t += dt
         kind, dt_name = "port", "f32"
-        what = f"oracle port of the reference path (torch CPU fp32, {threads} threads; baseline/_ref absent)"
+        what = f"oracle port of the reference path (torch CPU fp32, {threads} threads; oracle/_ref absent)"
     val = fl * steps / t / 1e12
     sample = f"{what}: fwd+bwd bs=1 S={S} H={Hc} d=128 non-causal, 4 simulated ring ranks per step"
     print(json.dumps({
@@ -298,26 +303,30 @@ def ring_parity(world, rank, dev, double_group):
             "cases": cases, "ok": not failed, "failed": failed, "max_abs_err": float(w.item())}
 
 
-def ref_ratio(world, S, causal, value):
-    """value / the UNMODIFIED reference's fwd+bwd TFLOPS/s on the same kind of box at the same (N, S, causal), as
-    measured by tools/ref_on_b200.py and committed in profiles/ref_on_b200_r02.json (None if not measured)."""
-    path = os.path.join(ROOT, "profiles", "ref_on_b200_r02.json")
-    if not os.path.exists(path):
-        return None
-    for ln in open(path):
-        try:
-            r = json.loads(ln)
-        except Exception:  # noqa: BLE001
-            continue
-        if r.get("n_gpus") == world and r.get("seq") == S and bool(r.get("causal")) == bool(causal):
-            return {"ratio": value / r["fwd_bwd_tflops"], "reference_tflops": r["fwd_bwd_tflops"],
-                    "source": "profiles/ref_on_b200_r02.json (tools/ref_on_b200.py, separate box of the same pool)"}
-    return None
+DUMP_TOTAL_ELEMS = 1 << 23  # fp32 elements over every file a run writes: 32 MiB, under the 64 MB budget
+
+
+def dump_outputs(out_dir, tensors, rank, world, n_runs, tag):
+    """Write each tensor as float32 .npy: DIR/<name>.npy, with _rank<r> appended when world > 1 and _<tag> (the
+    config) when a run has several configs.  The budget DUMP_TOTAL_ELEMS is shared by every tensor, rank and config
+    of the run; a tensor larger than its share is sampled at fixed positions (seed 0: the same for every run with
+    the same arguments)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = (f"_rank{rank}" if world > 1 else "") + (f"_{tag}" if n_runs > 1 else "")
+    share = DUMP_TOTAL_ELEMS // (len(tensors) * world * n_runs)
+    for name, t in tensors.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > share:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randint(0, flat.numel(), (share,), generator=g).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, f"{name}{sfx}.npy"), flat.float().cpu().numpy())
 
 
 def ncu_traffic(kernel, Sq, Sk, Hh, causal):
     """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of `kernel` at this launch shape from the
-    ncu --set full summary that tools/profile.sh regenerates (profiles/ncu_traffic.json); None when that shape was
+    ncu --set full summary stored in profiles/ncu_traffic.json; None when that shape was
     never captured -- never a literal."""
     path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if not os.path.exists(path):
@@ -338,7 +347,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--seq", type=int, default=262144, help="global sequence length")
+    ap.add_argument("--seq", type=int, default=None,
+                    help=f"global sequence length (default {SEQ_MULTI} on N > 1 GPUs, {SEQ_SINGLE} on one)")
     ap.add_argument("--causal", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
@@ -350,6 +360,10 @@ def main():
     ap.add_argument("--configs", default="", help="comma list of extra runs in the same process group, e.g. "
                     "'262144,524288c,1048576' (c = causal zigzag); one JSON line each (multi-GPU sessions are "
                     "expensive to start)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what the last one computed (O, dQ, dK, dV of every rank) to "
+                         "DIR/<name>[_rank<r>][_<config>].npy as float32: a fixed seeded sample, 32 MiB in all "
+                         "(split over ranks and configs)")
     ap.add_argument("--double-ring", type=int, default=0, metavar="L",
                     help="run over the hierarchical (double) ring with intra-node rings of L consecutive ranks "
                          "(reference benchmarks/benchmark.py --double_ring); default 0 = flat ring")
@@ -368,6 +382,8 @@ def main():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
     assert world == args.gpus, f"--gpus {args.gpus} but WORLD_SIZE={world}"
+    if args.seq is None:
+        args.seq = SEQ_MULTI if world > 1 else SEQ_SINGLE
     W = max(3, args.warmup)
     K = max(1, args.steps)
 
@@ -394,6 +410,7 @@ def main():
             m = re.fullmatch(r"(\d+)(c?)(?:b(\d+))?", c.strip())
             assert m, f"bad config token {c!r}"
             runs.append((int(m.group(1)), bool(m.group(2)), int(m.group(3) or B)))
+    args.n_runs = len(runs)
     for seq_i, causal_i, batch_i in runs:
         args.seq, args.causal, args.batch = seq_i, causal_i, batch_i
         _bench_one(args, world, rank, local, dev, W, K, ops, burst_attn_func)
@@ -454,13 +471,25 @@ def _bench_one(args, world, rank, local, dev, W, K, ops, burst_attn_func):
     ops.enable_timing(True)
     launches0 = ops.launches
     t_wall0 = time.time()
-    ms_step = timed(lambda: step(q, k, v, do), K)
+    last, n_done = {}, [0]
+
+    def timed_step():  # keeps the outputs of the LAST timed step only, and only when they are to be dumped
+        n_done[0] += 1
+        out = step(q, k, v, do)
+        if args.dump_outputs and n_done[0] == K:
+            last["out"] = out
+
+    ms_step = timed(timed_step, K)
     t_wall1 = time.time()
     launches = ops.launches - launches0
     torch.cuda.synchronize()
     kms = ops.kernel_ms()
     ops.enable_timing(False)
     clocks = sampler.stop(t_wall0, t_wall1)
+    if args.dump_outputs:
+        tag = f"S{S}{'c' if args.causal else ''}b{Bn}"
+        dump_outputs(args.dump_outputs, dict(zip(("o", "dq", "dk", "dv"), last.pop("out"))), rank, world,
+                     args.n_runs, tag)
     ms_fwd = timed(lambda: fwd_only(q, k, v), max(1, min(K, 3)))
 
     causal_div = 2.0 if args.causal else 1.0
@@ -477,7 +506,7 @@ def _bench_one(args, world, rank, local, dev, W, K, ops, burst_attn_func):
         # 10*Sq*Sk*H*D per round) / launches per step; non-causal: exactly 10*S_loc^2*H*D per ring round
         fl_launch = flops(S, "bwd", Bn) / causal_div / world / (n_l / K)
         ach = fl_launch / (tot_ms / n_l * 1e-3) / 1e12
-        # DRAM traffic per launch: read from the per-shape ncu --set full summary tools/profile.sh regenerates
+        # DRAM traffic per launch: read from the per-shape ncu --set full summary, when one is stored
         # (profiles/ncu_traffic.json), for the launch shape this run actually used; None if never captured
         shp = ops.dominant_shape("bwd_chunk_kernel")
         traffic, traffic_src = ncu_traffic("bwd_chunk_kernel", *shp) if shp else (None, None)
@@ -590,11 +619,10 @@ def _bench_one(args, world, rank, local, dev, W, K, ops, burst_attn_func):
                                    f"{'local kernel, no ring' if world == 1 else f'{world}-rank ring over ' + ('copy engines + CUDA IPC' if _ring_transport() == 'ce' else 'NCCL')}"
                                    f"{f' (double ring, intra {args.double_ring})' if args.double_ring and world > 1 else ''}",
                        "global_batch": Bn, "seq_len": S, "parallelism": f"sp{world}",
-                       "l2": "inputs (>= 256 MiB per tensor per rank) exceed the 126 MB L2; no flush needed"},
+                       "l2": "inputs (>= 256 MiB per tensor per rank) exceed the 50 MB L2; no flush needed"},
             "value_per_gpu": value / world, "fwd_tflops": fwd_tflops, "fwd_ms": ms_fwd,
             "gpu_launches": int(tot_launch.item()), "clocks": clocks, "e2e": e2e, "roofline": roof, "overlap": overlap,
             "cpu_baseline": cpu, "parity": getattr(args, "parity", None), "comm_ab": ab,
-            "vs_reference_on_b200": ref_ratio(world, S, args.causal, value),
         }
         print(json.dumps(line), flush=True)
 

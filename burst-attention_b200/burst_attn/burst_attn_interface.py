@@ -8,7 +8,7 @@ ring schedules (forward: K/V rotate, :214-242; backward: the Q-bundle
 (delta, dO, Q, lse) rotates and the partial dQ rides one hop behind it,
 :291-396), output dtype, the assertion that causal needs flash == "cuda".
 
-What is B200-native instead (DESIGN.md): every round is ONE kernel launch of the
+What is H100-native instead (DESIGN.md): every round is ONE kernel launch of the
 C-ABI library (carried (O, lse) state and fp32 dQ/dK/dV accumulation fused into
 the tile kernels; half-sequence and shifted cases are pointer/length views or a
 causal offset, never ``.contiguous()`` copies); user tensors are never used as
@@ -60,8 +60,7 @@ def get_partition_id(double_group, r):
 
 
 # Hierarchical ring over NCCL: on when the caller passes double_group (BA_DOUBLE_RING=0 forces the flat ring over
-# process_group).  `RING_CHECK_DOUBLE=2,4 torchrun tests/ring_check.py` passed on 8 x B200 for intra-node rings of 2
-# and of 4 (profiles/ring_check_r02_n8_nccl.txt).
+# process_group).  `RING_CHECK_DOUBLE=2,4 torchrun tests/ring_check.py` checks it for intra-node rings of 2 and of 4.
 _DOUBLE_RING_DEFAULT = "1"
 
 
@@ -114,10 +113,8 @@ def _nbytes(t) -> int:
 
 def _l2_block() -> int:
     """Rows/keys per sub-launch.  One (batch, head) slice of 32768 keys is 16 MiB of K+V (or 32 MiB of
-    Q, dO and fp32 dQ in the backward), so the streamed operands of a launch stay resident in B200's
-    126 MB L2 while all CTAs of a head sweep them -- measured on one GPU at S=262144: forward +7 %
-    (1147 vs 1069 TFLOP/s), backward unchanged, compared with one launch over the whole sequence.  The multi-GPU rounds at S_local <= 49152 are
-    unaffected.  BA_L2_BLOCK overrides (tests use tiny blocks)."""
+    Q, dO and fp32 dQ in the backward), so the streamed operands of a launch can stay resident in H100's
+    50 MB L2 while all CTAs of a head sweep them.  The multi-GPU rounds at S_local <= 49152 are unaffected.  BA_L2_BLOCK overrides (tests use tiny blocks)."""
     return int(os.environ.get("BA_L2_BLOCK", "32768"))
 
 
@@ -500,7 +497,7 @@ def _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, dete
 
 
 def _pad_head_dim(ops, tensors):
-    """The sm_100a tile kernels exist for head_dim 64 and 128 (``ops.tile_head_dims``; the reference's
+    """The sm_90a tile kernels exist for head_dim 64 and 128 (``ops.tile_head_dims``; the reference's
     CPU-runnable configuration C1 has 64, its benchmarks 128).  Any other head_dim <= 128 is run exactly by
     zero-padding the last axis once per call up to the next tile width: padded Q/K columns add 0 to every score,
     padded V columns produce output columns that are exactly 0 and are sliced off, and the same holds for
@@ -520,7 +517,7 @@ def _unpad(t, D):
 
 def _op_forward(ctx, q, k, v, mode):
     ctx.host = False
-    if q.device.type == "cpu" and getattr(get_ops(), "name", "") == "sm100":  # (tests inject CPU chunk operators)
+    if q.device.type == "cpu" and getattr(get_ops(), "name", "") == "sm90":  # (tests inject CPU chunk operators)
         # host-resident operands (pinned CPU tensors, one rank): copies stream under the kernels (host_stream.py)
         from . import host_stream
         if not host_stream.is_host_call(q, k, v):

@@ -23,7 +23,7 @@ def _dims(t: torch.Tensor, seq_dim: int):
 
 
 class NativeOps:
-    name = "sm100"
+    name = "sm90"
     tile_head_dims = (64, 128)  # head dims the tile kernels are built for; the drivers zero-pad others up
 
     def __init__(self):

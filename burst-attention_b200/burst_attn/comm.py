@@ -24,8 +24,8 @@ A ``Ring`` here is always ONE ring over ONE group.  The reference's intra/inter
 them -- intra-node hops, inter-node prefetch of the block that starts the next
 cycle, inter-node chain of the dQ node sums (burst_attn_interface.py:
 ``_ring_forward_hier`` / ``_bwd_rounds_hier``) -- so each level has its own
-communicator and side stream and is awaited independently.  8 x B200 on one
-NVSwitch is a uniform fabric where the flat ring is as good; the hierarchy is for
+communicator and side stream and is awaited independently.  8 GPUs on one
+NVSwitch are a uniform fabric where the flat ring is as good; the hierarchy is for
 W spanning several NVLink domains.
 """
 from __future__ import annotations
@@ -218,9 +218,8 @@ def destroy_rings() -> None:
 def default_transport() -> str:
     """Transport of a flat ring when the caller does not name one: ``BA_RING_TRANSPORT`` if set; otherwise the copy
     engines (``ce``) when every rank of the job runs on this node -- torchrun's LOCAL_WORLD_SIZE equals the world
-    size -- and NCCL in every other case (several nodes, or a launcher that does not say).  Measured on 8 x B200
-    (profiles/README_r02.md): ce 8181 vs nccl 8091 TFLOPS/s at S = 262144 (NCCL's SM-resident send/recv kernels slow
-    the tile kernels down while they co-run) and 7770 vs 6178 at S = 65536 (there NCCL's hop is exposed)."""
+    size -- and NCCL in every other case (several nodes, or a launcher that does not say).  The copy engines take no
+    SMs, whereas NCCL's SM-resident send/recv kernels slow the tile kernels down while they co-run."""
     env = os.environ.get("BA_RING_TRANSPORT")
     if env:
         return env

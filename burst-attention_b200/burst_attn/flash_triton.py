@@ -2,7 +2,7 @@
 (burst_attn/flash_triton.py:1013-1160: ``flash_attn_func``, ``flash_attn_kvpacked_func``,
 ``flash_attn_qkvpacked_func``; layout [batch, seqlen, nheads, headdim], ``causal`` bottom-right aligned like the
 Triton kernel's ``seqlen_k - seqlen_q`` offset).  The reference keeps a vanilla Triton FlashAttention copy there
-that its ring op never calls; here the three wrappers run the same sm_100a tile kernels as the ring (one local
+that its ring op never calls; here the three wrappers run the same sm_90a tile kernels as the ring (one local
 "round", no communication), reading Q / K / V straight out of the packed tensor through strided views (TMA takes
 the strides; nothing is unpacked or copied on the way in).
 
@@ -31,7 +31,7 @@ def _key_bias(bias, q, k):
         return None
     B, H, Sk = q.shape[0], q.shape[2], k.shape[1]
     if bias.dim() != 4 or bias.shape[2] != 1 or bias.shape[3] != Sk or bias.shape[1] != H or bias.shape[0] not in (1, B):
-        raise NotImplementedError(f"only a per-key bias of shape (batch | 1, {H}, 1, {Sk}) is supported by the sm_100a "
+        raise NotImplementedError(f"only a per-key bias of shape (batch | 1, {H}, 1, {Sk}) is supported by the sm_90a "
                                   f"tile kernels, got {tuple(bias.shape)}")
     b3 = bias.detach().to(torch.float32).reshape(bias.shape[0], H, Sk).contiguous()
     return b3.expand(B, H, Sk)

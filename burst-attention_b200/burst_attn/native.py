@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library ``libburst_attn_b200.so`` (include/burst_attn_b200.h).
 
 There is deliberately NO fallback: if the shared library is missing or the
-device is not sm_100, every entry point raises.  PyTorch is used only for
+device is not sm_90 (H100), every entry point raises.  PyTorch is used only for
 device memory and streams (``tensor.data_ptr()``, ``torch.cuda.current_stream()``).
 """
 from __future__ import annotations
@@ -46,7 +46,7 @@ _EXPORTS = (
     "ba_ring_arena_connect",
 )
 SELFTEST_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libburst_attn_b200_selftest.so")
-_SELFTEST_EXPORTS = ("ba_selftest_last_error", "ba_selftest", "ba_ubench")
+_SELFTEST_EXPORTS = ("ba_selftest_last_error", "ba_selftest")
 
 
 def exported_symbols() -> Sequence[str]:
@@ -120,8 +120,6 @@ def selftest_lib() -> ctypes.CDLL:
         L = ctypes.CDLL(SELFTEST_LIB_PATH)
         i, vp = ctypes.c_int, ctypes.c_void_p
         L.ba_selftest_last_error.restype = ctypes.c_char_p
-        L.ba_ubench.restype = i
-        L.ba_ubench.argtypes = [i, i, i, ctypes.POINTER(ctypes.c_int64), vp]
         L.ba_selftest.restype = i
         L.ba_selftest.argtypes = [i, vp, vp, vp, i, vp]
         _selftest_lib = L

@@ -3,7 +3,7 @@
 // All are one pass over their operands with 16-byte accesses; head dim D = 64 or 128: a (row, head) pair is
 // covered by D/16 (delta), D/8 (cast) or D/4 (accumulate) consecutive threads (`lpr`, a power of two).
 #include "host_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace ba {
 

@@ -88,8 +88,8 @@ extern "C" int ba_device_check(void) {
   int major = 0, minor = 0;
   BA_CHECK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   BA_CHECK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 10) {
-    ba::set_error("burst_attn_b200 needs an sm_100 (B200) device, found sm_%d%d", major, minor);
+  if (major != 9 || minor != 0) {
+    ba::set_error("burst_attn_b200 needs an sm_90 (H100) device, found sm_%d%d", major, minor);
     return BA_ERR_UNSUPPORTED;
   }
   return BA_OK;

@@ -1,7 +1,7 @@
 // Copy-engine ring transport (optional, same-node rings): one hop = peer cudaMemcpyAsync pushes over
 // NVLink executed by the copy engines -- no SMs, so the hop does not compete with the tile kernels the
-// way NCCL's SM-resident send/recv kernels do (profiles/README.md: 24.5 % of the step exposed at
-// S_local = 8192 with NCCL).  Same post/wait contract as the NCCL transport (ring_nccl.cu).
+// way NCCL's SM-resident send/recv kernels do (which matters most for short shards, where the hop is
+// exposed).  Same post/wait contract as the NCCL transport (ring_nccl.cu).
 //
 // Receive buffers live in a ring-owned arena that every rank carves identically (a symmetric heap), so
 // "my destination's offset in my arena" is also the offset to write at in the next rank's arena, which

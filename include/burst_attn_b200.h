@@ -1,4 +1,4 @@
-/* burst_attn_b200 -- C ABI of the B200-native chunk operators and ring transport
+/* burst_attn_b200 -- C ABI of the H100-native (sm_90a) chunk operators and ring transport
  * that replace the reference's "operator boundary" (SURVEY.md 8b):
  *
  *   attn_forward / attn_backward      burst_attn/burst_attn_interface.py:40-93
@@ -63,7 +63,7 @@ typedef struct {
 } ba_rowstat;
 
 const char* ba_last_error(void);
-/* Library / device capability probe: returns BA_OK when the current device is sm_100. */
+/* Library / device capability probe: returns BA_OK when the current device is sm_90 (H100). */
 int ba_device_check(void);
 int ba_version(void);
 
@@ -83,8 +83,8 @@ int ba_fwd_chunk(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_
  * of the reference's LAO tile, burst_attn/lao.py:102-105,155-173; its ring op always passes bias = None,
  * burst_attn_interface.py:223,316, so this serves the single-GPU wrappers of burst_attn/flash_triton.py).
  * key_bias: fp32 [B,H,Sk] view (stride_b may be 0 to broadcast over the batch; ptr NULL = no bias).  -inf entries
- * mask a key.  The forward adds it on the tensor core (one extra K = 16 step per score tile), the backward in the
- * exponent's FMA; no gradient is produced for the bias (neither does the reference: flash_triton.py:1046).       */
+ * mask a key.  Both kernels add it in the exponent's FMA; no gradient is produced for the bias (neither does the
+ * reference: flash_triton.py:1046).                                                                              */
 int ba_fwd_chunk_bias(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc, ba_rowstat lse,
                       ba_tensor4 o_out, int B, int Sq, int Sk, int H, int D, float scale, int mask_mode,
                       int causal_offset, int flags, int dtype, void* stream);

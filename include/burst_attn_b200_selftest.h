@@ -1,4 +1,4 @@
-/* burst_attn_b200_selftest -- diagnostics of the sm_100a building blocks.  NOT part of the drop-in boundary:
+/* burst_attn_b200_selftest -- diagnostics of the sm_90a building blocks.  NOT part of the drop-in boundary:
  * these entry points live in their own library (libburst_attn_b200_selftest.so) that only tests/ and tools/ load.
  * Same conventions as burst_attn_b200.h (status codes, ba_last_error of the main library is not shared: this
  * library exports ba_selftest_last_error).                                                                   */
@@ -13,25 +13,13 @@ extern "C" {
 
 const char* ba_selftest_last_error(void);
 
-/* ---- self tests of the sm_100a building blocks (tests/ only) --------------------
- * mode 0: S[128,128] fp32 = A[128,128] * B[128,128]^T through TMA + tcgen05 SS MMA
- * mode 1: O[128,128] fp32 = P[128,128] * V[128,128] with P staged in TMEM (TS MMA)
+/* ---- self tests of the sm_90a building blocks (tests/ only) --------------------
+ * mode 0: S[128,128] fp32 = A[128,128] * B[128,128]^T through TMA + wgmma SS (both operands K-major)
+ * mode 1: O[128,128] fp32 = P[128,128] * V[128,128] with P in registers (wgmma RS, V MN-major)
  * mode 2: raw dump of a TMA-loaded 128x64 SWIZZLE_128B box (16 KiB)
  * mode 3: out = A^T * B with both operands MN-major (backward's dQ path)
- * a, b: dtype [128,128] row-major; out: fp32 [128,128] (mode 2: 8192 x 16-bit).
- * mode 4/5: CTA-pair (cta_group::2, cluster of 2) SS / TS GEMM: a [256,128], b [128,128], out fp32 [256,128].
- * mode 6: TMEM layout probe of an M = 128 cta_group::2 MMA (a [128,128]; out = raw [2][128 lanes][128 cols] dump,
- *         12345.0 where nothing was written); mode 7: mode 4 with the B halves delivered through DSMEM stores
- *         by the peer CTA (tools/probe_pair.py).                                                              */
+ * a, b: dtype [128,128] row-major; out: fp32 [128,128] (mode 2: 8192 x 16-bit).                               */
 int ba_selftest(int mode, const void* a, const void* b, void* out, int dtype, void* stream);
-
-/* ---- micro-benchmarks of the sm_100a building blocks (tools/ubench.py only) -------------------
- * Runs one timing kernel (`grid` CTAs, or CTA pairs for the cta_group::2 modes) and returns device clock
- * cycles in out4_host[0] (and [1] for mode 14); synchronises the stream.  Modes: 0-4 tcgen05.mma chains of
- * `iters` dispatches (SS/TS, N = 128/256/64), 5-7 the same on CTA pairs (M = 256), 8-10 and 16 tcgen05.ld / st
- * groups, 11 MUFU ex2, 12 single-MMA latency, 13 / 15 cluster-remote arrive and multicast-commit round
- * trips, 14 a TS chain with tcgen05.ld traffic beside it (csrc/ubench_sm100.cu).                       */
-int ba_ubench(int mode, int iters, int grid, int64_t* out4_host, void* stream);
 
 #ifdef __cplusplus
 }

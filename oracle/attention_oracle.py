@@ -7,7 +7,7 @@ library is missing.
 
 This is a restatement (not a copy) of the reference's algorithm in plain
 torch-on-CPU tensor arithmetic, each function citing the reference lines it
-follows (paths relative to /root/reference).  It is pinned against the
+follows (paths relative to the reference checkout).  It is pinned against the
 reference itself by ``tests/golden/make_golden.py`` (reference imported in the
 build container with a ``bmtrain`` stub) -> ``tests/golden/*.npz`` and checked
 by ``tests/test_oracle_golden.py``.

@@ -1,13 +1,13 @@
-"""Generate golden vectors by RUNNING THE REFERENCE (MayDomine/Burst-Attention at
-/root/reference) on CPU in the build container.  The reference cannot travel to
-the GPU box, so its outputs are committed as small .npz fixtures next to this
+"""Generate golden vectors by RUNNING THE REFERENCE (a checkout of
+MayDomine/Burst-Attention) on CPU.  The reference is not a dependency of this
+project, so its outputs are committed as small .npz fixtures next to this
 script; tests/test_oracle_golden.py pins oracle/attention_oracle.py to them.
 
 The reference imports `bmtrain` (absent here) at module scope
 (burst_attn_interface.py:1, comm.py:2-5); a stub module is injected -- no
 reference source is modified or copied.
 
-Run:  python tests/golden/make_golden.py      (needs /root/reference)
+Run:  python tests/golden/make_golden.py <path of the reference checkout>
 """
 import os
 import sys
@@ -17,7 +17,6 @@ import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
 
 
 def _stub_bmtrain():
@@ -36,17 +35,56 @@ def _stub_bmtrain():
     bmt.distributed, bmt.nccl = d, nccl
 
 
-def main():
+def ring_vectors(bu):
+    """The reference's device-agnostic chunk path (inter_normal_attn / _backward, burst_utils.py:42-100) over a ring
+    of W ranks simulated in one process, schedule of OpBurstAttn.forward/backward (burst_attn_interface.py:214-248,
+    291-396) without the transport; layout [B,H,S,D], fp32.  Inputs are fp16-representable (stored losslessly as
+    fp16); the outputs are stored at a fixed, seeded sample of 512 positions per tensor."""
+    g = torch.Generator().manual_seed(0)
+    B, H, S, D = 1, 1, 64, 32
+    q, k, v, do = (torch.randn(B, H, S, D, generator=g).half().float() for _ in range(4))
+    idx = torch.randperm(B * H * S * D, generator=g)[:512].sort().values
+    out = dict(ring_q=q.half(), ring_k=k.half(), ring_v=v.half(), ring_do=do.half(), ring_idx=idx,
+               ring_scale=torch.tensor(D ** -0.5))
+    for W in (1, 4):
+        qs, ks, vs, dos = (t.chunk(W, dim=2) for t in (q, k, v, do))
+        outs, lses = [], []
+        for i in range(W):
+            m_i = lse_i = acc_o = None
+            for r in range(W):  # round r: rank i holds the K/V shard of rank (i - r) mod W
+                j = (i - r) % W
+                acc_o, m_i, lse_i = bu.inter_normal_attn(qs[i], ks[j], vs[j], m_i, lse_i, acc_o, D ** -0.5, None)
+            outs.append(acc_o * torch.exp(m_i - lse_i))
+            lses.append(lse_i)
+        dqs = [torch.zeros_like(t) for t in qs]
+        dks = [torch.zeros_like(t) for t in ks]
+        dvs = [torch.zeros_like(t) for t in vs]
+        deltas = [(outs[i] * dos[i]).sum(-1, keepdim=True) for i in range(W)]
+        for j in range(W):  # K/V at home on rank j, the Q-bundle of rank i visits
+            for r in range(W):
+                i = (j - r) % W
+                buf = torch.empty_like(qs[i])
+                bu.inter_normal_attn_backward(dos[i], qs[i], ks[j], vs[j], deltas[i], lses[i], buf, dks[j], dvs[j],
+                                              D ** -0.5, None)
+                dqs[i] += buf
+        for name, parts in (("o", outs), ("dq", dqs), ("dk", dks), ("dv", dvs)):
+            out[f"ring_W{W}_{name}"] = torch.cat(parts, dim=2).reshape(-1)[idx]
+    np.savez_compressed(os.path.join(HERE, "reference_ring.npz"), **{k_: v_.numpy() for k_, v_ in out.items()})
+
+
+def main(ref):
     _stub_bmtrain()
-    sys.path.insert(0, REF)
+    sys.path.insert(0, ref)
     import burst_attn.burst_utils as bu
     import burst_attn.burst_attn_interface as bi
+
+    ring_vectors(bu)
 
     torch.manual_seed(20260922)
     out = {}
 
     # ---- 1. chunked forward chain through inter_normal_attn (burst_utils.py:42-74)
-    B, H, S, D, W = 1, 2, 256, 64, 4
+    B, H, S, D, W = 1, 1, 64, 32, 4
     scale = 1.0 / D ** 0.5
     q = torch.randn(B, H, S, D)
     k = torch.randn(B, H, S, D)
@@ -79,7 +117,7 @@ def main():
                bwd_dk=torch.cat(dk_parts, 2), bwd_dv=torch.cat(dv_parts, 2))
 
     # ---- 3. LSE merge cuda_scale_out_lse_helper (burst_utils.py:20-33)
-    Bm, Sm, Hm, Dm = 2, 48, 3, 16
+    Bm, Sm, Hm, Dm = 1, 16, 2, 8
     o = torch.randn(Bm, Sm, Hm, Dm)
     lse = torch.randn(Bm, Sm, Hm, 1) * 3
     o_new = torch.randn(Bm, Sm, Hm, Dm)
@@ -117,9 +155,9 @@ def main():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         os.environ.setdefault("MASTER_PORT", "29577")
         dist.init_process_group("gloo", rank=0, world_size=1)
-        qq = torch.randn(1, 2, 128, 32)
-        kk = torch.randn(1, 2, 128, 32)
-        vv = torch.randn(1, 2, 128, 32)
+        qq = torch.randn(1, 1, 32, 16)
+        kk = torch.randn(1, 1, 32, 16)
+        vv = torch.randn(1, 1, 32, 16)
         oo = bi.burst_attn_func(qq, kk, vv, None, None, False)
         out.update(op_q=qq, op_k=kk, op_v=vv, op_o=oo)
         dist.destroy_process_group()
@@ -132,4 +170,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

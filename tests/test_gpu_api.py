@@ -46,7 +46,7 @@ def test_normal_layout_flash_none():
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 def test_flash_triton_noncausal(dtype):
     """flash="triton" (reference: inter_flash_attn_triton / _backward_triton, burst_utils.py:103-146) selects the
-    same sm_100a tile kernels in the flash layout [B,S,N,H]; non-causal is the only mode the reference allows."""
+    same sm_90a tile kernels in the flash layout [B,S,N,H]; non-causal is the only mode the reference allows."""
     torch.manual_seed(2)
     b, s, n, d = 2, 384, 4, 128
     q, k, v, do = (torch.randn(b, s, n, d, device="cuda", dtype=dtype) for _ in range(4))

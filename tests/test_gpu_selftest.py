@@ -1,5 +1,5 @@
-"""sm_100a building blocks (TMA box/swizzle, UMMA descriptors, TMEM lane mapping,
-TS-form MMA) checked one by one against torch on the GPU."""
+"""sm_90a building blocks (TMA box/swizzle, wgmma descriptors, accumulator fragment,
+register-A form of wgmma) checked one by one against torch on the GPU."""
 import pytest
 import torch
 
@@ -35,7 +35,7 @@ def test_ss_kmajor_gemm(ab, dtype):
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
-def test_ts_gemm_p_in_tmem(ab, dtype):
+def test_rs_gemm_p_in_registers(ab, dtype):
     a, b = (t.to(dtype) for t in ab)
     out = selftest(1, a, b)
     torch.testing.assert_close(out, a.float() @ b.float(), rtol=1e-3, atol=1e-2)
@@ -45,21 +45,3 @@ def test_ss_mnmajor_gemm(ab):
     a, b = ab
     out = selftest(3, a, b)
     torch.testing.assert_close(out, a.float().t() @ b.float(), rtol=1e-3, atol=1e-2)
-
-
-def test_cta_pair_ss_gemm():
-    """cta_group::2: one M=256 MMA over a 2-CTA cluster, each CTA holding half of B (building block of the
-    planned CTA-pair kernels)."""
-    torch.manual_seed(1)
-    a = torch.randn(256, 128, device="cuda").to(torch.bfloat16)
-    b = torch.randn(128, 128, device="cuda").to(torch.bfloat16)
-    out = selftest(4, a, b)
-    torch.testing.assert_close(out, a.float() @ b.float().t(), rtol=1e-3, atol=1e-2)
-
-
-def test_cta_pair_ts_gemm():
-    torch.manual_seed(2)
-    a = torch.randn(256, 128, device="cuda").to(torch.bfloat16)
-    b = torch.randn(128, 128, device="cuda").to(torch.bfloat16)
-    out = selftest(5, a, b)
-    torch.testing.assert_close(out, a.float() @ b.float(), rtol=1e-3, atol=1e-2)

@@ -36,7 +36,7 @@ def test_library_exports_every_declared_symbol(nat):
 
 
 def test_selftest_library_is_separate_from_the_product(nat):
-    """Diagnostics (ba_selftest, ba_ubench) live in their own header and library, not in the drop-in boundary."""
+    """Diagnostics (ba_selftest) live in their own header and library, not in the drop-in boundary."""
     hdr = open(os.path.join(ROOT, "include", "burst_attn_b200_selftest.h")).read()
     declared = sorted(set(re.findall(r"\b(ba_[a-z0-9_]+)\s*\(", hdr)))
     assert declared == sorted(nat._SELFTEST_EXPORTS)
@@ -44,7 +44,7 @@ def test_selftest_library_is_separate_from_the_product(nat):
     for name in declared:
         assert hasattr(T, name), name
     L = ctypes.CDLL(nat.LIB_PATH)
-    for name in ("ba_selftest", "ba_ubench"):
+    for name in ("ba_selftest", "ba_selftest_last_error"):
         assert not hasattr(L, name), f"{name} must not be exported by the product library"
 
 

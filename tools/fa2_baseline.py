@@ -1,5 +1,5 @@
 """Informational baseline on the same box: the kernels the REFERENCE runs on this path --
-flash-attn 2.8.x `_flash_attn_forward/_backward` (FA2, mma.sync SASS for sm_100; what
+flash-attn 2.8.x `_flash_attn_forward/_backward` (FA2, mma.sync SASS; what
 burst_utils.py:149-249 calls) -- timed on the bench shapes.  flash_attn is an installed library,
 not part of this repo's product path; nothing here is used by bench.py's value."""
 import json

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Launch ONE tile kernel at a given launch shape a few times (for ncu: `-k regex:<kernel> -s 1 -c 1`).
+"""Launch ONE tile kernel at a given launch shape a few times (for a profiler run on one kernel).
   python tools/launch_one.py --kernel bwd --Sq 32768 --Sk 32768 [--H 32] [--causal] [--off 0] [--n 3] [--time]
 Inputs are N(0,1) bf16; lse/delta come from a real forward of the same shape when it is cheap, else plausible
 constants (timing and traffic do not depend on them)."""
