@@ -187,7 +187,9 @@ def _bwd_round(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, caus
 def _check_inputs(q, k, v, seq_dim):
     assert q.dim() == 4 and k.shape == v.shape and q.shape[0] == k.shape[0] and q.shape[3] == k.shape[3], \
         "q, k, v must be 4-D with matching batch and head_dim"
-    assert q.shape[3 - seq_dim] == k.shape[3 - seq_dim], "q and k/v must have the same number of heads"
+    hq, hkv = q.shape[3 - seq_dim], k.shape[3 - seq_dim]
+    assert hkv > 0 and hq % hkv == 0, \
+        f"the number of q heads ({hq}) must be a multiple of the number of k/v heads ({hkv})"
     assert q.dtype == k.dtype == v.dtype, "q, k, v must share a dtype"
 
 

@@ -9,7 +9,9 @@ methods to exercise the ring schedules on CPU/gloo; the product never does.)
 
 All tensors are 4-D with head_dim last and contiguous; ``seq_dim`` says which
 axis is the sequence (1: flash layout [B,S,H,D]; 2: normal layout [B,H,S,D]).
-lse / delta are fp32 [B,H,S].
+lse / delta are fp32 [B,H,S].  K and V (and dK / dV) may have fewer heads than Q
+(grouped-query attention: query head h reads K/V head h // (Hq // Hkv)); the number
+of K/V heads is taken from ``k``.
 """
 from __future__ import annotations
 
@@ -68,14 +70,15 @@ class NativeOps:
 
     # ---- forward round: fold chunk (k, v) into (o_acc, lse); on last write o_out
     def fwd_chunk(self, q, k, v, o_acc, lse, o_out, scale, causal, causal_offset, first, last, seq_dim, bias=None):
-        """bias: optional fp32 [B|1, H, Sk] additive bias per key (expanded views with stride 0 over the batch are fine)."""
+        """bias: optional fp32 [B|1, H, Sk] additive bias per key (expanded views with stride 0 over the batch are fine),
+        indexed by the query head."""
         B, Sq, H, D = _dims(q, seq_dim)
-        Sk = k.shape[seq_dim]
+        Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         flags = (_n.BA_FWD_FIRST if first else 0) | (_n.BA_FWD_LAST if last else 0)
         e0 = self._t0(q.device)
-        rc = self.lib.ba_fwd_chunk_bias(
+        rc = self.lib.ba_fwd_chunk_gqa(
             _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(bias), _n.t4(o_acc, seq_dim), _n.rs(lse),
-            _n.t4(o_out, seq_dim), B, Sq, Sk, H, D, float(scale),
+            _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale),
             _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset), flags,
             _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
         _n.check(rc, "ba_fwd_chunk")
@@ -97,11 +100,12 @@ class NativeOps:
     def bwd_chunk(self, d_o, q, k, v, delta, lse, dq_acc, dk_acc, dv_acc, scale, causal, causal_offset, seq_dim,
                   deterministic=False, bias=None):
         B, Sq, H, D = _dims(q, seq_dim)
-        Sk = k.shape[seq_dim]
+        Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         e0 = self._t0(q.device)
-        rc = self.lib.ba_bwd_chunk_bias(
+        rc = self.lib.ba_bwd_chunk_gqa(
             _n.t4(d_o, seq_dim), _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(delta), _n.rs(lse),
-            _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, D, float(scale),
+            _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv, D,
+            float(scale),
             _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset), 1 if deterministic else 0,
             _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
         _n.check(rc, "ba_bwd_chunk")

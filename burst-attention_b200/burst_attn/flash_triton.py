@@ -12,6 +12,11 @@ the strides; nothing is unpacked or copied on the way in).
 per-thread scalar in the exponent's FMA).  The "matrix" form ``(.., seqlen_q, seqlen_k)`` is not supported (at the
 sequence lengths this path is built for it does not fit memory) and raises.  As in the reference no gradient
 flows into the bias.
+
+Grouped-query / multi-query attention as in flash-attn: ``flash_attn_func`` and ``flash_attn_kvpacked_func`` accept
+K/V with ``nheads_k`` heads where ``nheads_k`` divides ``nheads``; query head ``h`` attends with K/V head
+``h // (nheads // nheads_k)``, and dK / dV come back with ``nheads_k`` heads (summed over each group).  A per-key bias
+is still ``(batch | 1, nheads, 1, seqlen_k)``, one row per query head.
 """
 from __future__ import annotations
 
@@ -73,12 +78,19 @@ def _check(bias, *ts):
         assert t.stride(-1) == 1, "the head_dim axis must be contiguous"
 
 
+def _check_heads(q, k):
+    hq, hkv = q.shape[2], k.shape[2]
+    assert hkv > 0 and hq % hkv == 0, f"nheads ({hq}) must be a multiple of nheads_k ({hkv})"
+
+
 class FlashAttnFunc(torch.autograd.Function):
-    """q: (batch, seqlen_q, nheads, headdim); k, v: (batch, seqlen_k, nheads, headdim)  (reference :1122-1168)."""
+    """q: (batch, seqlen_q, nheads, headdim); k, v: (batch, seqlen_k, nheads_k, headdim), nheads_k | nheads
+    (reference :1122-1168)."""
 
     @staticmethod
     def forward(ctx, q, k, v, bias=None, causal=False, softmax_scale=None):
         _check(bias, q, k, v)
+        _check_heads(q, k)
         ctx.bias = _key_bias(bias, q, k)
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, k, v, causal, softmax_scale, ctx.bias)
         ctx.save_for_backward(*saved, out, lse)
@@ -93,11 +105,13 @@ class FlashAttnFunc(torch.autograd.Function):
 
 
 class FlashAttnKVPackedFunc(torch.autograd.Function):
-    """q: (batch, seqlen_q, nheads, headdim); kv: (batch, seqlen_k, 2, nheads, headdim)  (reference :1073-1119)."""
+    """q: (batch, seqlen_q, nheads, headdim); kv: (batch, seqlen_k, 2, nheads_k, headdim), nheads_k | nheads
+    (reference :1073-1119)."""
 
     @staticmethod
     def forward(ctx, q, kv, bias=None, causal=False, softmax_scale=None):
         _check(bias, q, kv)
+        _check_heads(q, kv[:, :, 0])
         ctx.bias = _key_bias(bias, q, kv[:, :, 0])
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, kv[:, :, 0], kv[:, :, 1], causal,
                                                                           softmax_scale, ctx.bias)

@@ -40,7 +40,7 @@ _lib = None
 
 _EXPORTS = (
     "ba_last_error", "ba_device_check", "ba_version", "ba_fwd_chunk", "ba_fwd_chunk_bias", "ba_bwd_delta", "ba_bwd_chunk",
-    "ba_bwd_chunk_bias",
+    "ba_bwd_chunk_bias", "ba_fwd_chunk_gqa", "ba_bwd_chunk_gqa",
     "ba_cast_from_f32", "ba_accumulate_f32", "ba_ring_unique_id", "ba_ring_create", "ba_ring_post",
     "ba_ring_wait", "ba_ring_rank", "ba_ring_world", "ba_ring_destroy", "ba_ring_arena_create",
     "ba_ring_arena_connect",
@@ -77,6 +77,12 @@ def lib() -> ctypes.CDLL:
     L.ba_bwd_chunk_bias.restype = i
     L.ba_bwd_chunk_bias.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_rowstat, ba_rowstat,
                                     ba_tensor4, ba_tensor4, ba_tensor4, i, i, i, i, i, f, i, i, i, i, vp]
+    L.ba_fwd_chunk_gqa.restype = i
+    L.ba_fwd_chunk_gqa.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_tensor4, ba_rowstat, ba_tensor4,
+                                   i, i, i, i, i, i, f, i, i, i, i, vp]
+    L.ba_bwd_chunk_gqa.restype = i
+    L.ba_bwd_chunk_gqa.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_rowstat, ba_rowstat,
+                                   ba_tensor4, ba_tensor4, ba_tensor4, i, i, i, i, i, i, f, i, i, i, i, vp]
     L.ba_bwd_delta.restype = i
     L.ba_bwd_delta.argtypes = [ba_tensor4, ba_tensor4, ba_rowstat, i, i, i, i, i, vp]
     L.ba_bwd_chunk.restype = i

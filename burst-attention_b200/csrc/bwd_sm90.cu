@@ -7,9 +7,12 @@
 // delta = rowsum(O*dO) and the final lse are inputs (they travel with the
 // Q-bundle), so O itself is never read here.
 //
-// One CTA owns one 128-key block of the home K/V chunk for one (batch, head) and loops over the 64-row blocks of
-// the visiting Q-bundle.  Warpgroup 0 is the TMA producer (K, V once; Q, dO and the row statistics per Q block,
-// 2 stages); warpgroups 1 and 2 own 64 keys each and keep their dK, dV accumulators in registers:
+// One CTA owns one 128-key block of the home K/V chunk for one (batch, K/V head) and loops over the G query heads
+// that share that K/V head (grouped-query attention; G = 1 for MHA) and, for each, over the 64-row blocks of the
+// visiting Q-bundle: G x n_it steps, one pipeline whose stages and mbarrier phases run on across heads.
+// Warpgroup 0 is the TMA producer (K, V once; Q, dO and the row statistics per step, 2 stages); warpgroups 1 and 2
+// own 64 keys each and keep their dK, dV accumulators in registers across all G heads, so the epilogue does a
+// single read-modify-write of dk_acc / dv_acc per CTA (no atomics; dK / dV stay deterministic):
 //   S^T  = K_w Q_i^T,  dP^T = V_w dO_i^T      (wgmma SS m64n64, K-major operands)
 //   P^T  = exp2(S^T c [+ bias] - lse2),  dS^T = P^T o (dP^T - delta)     (registers, thread = 2 key rows)
 //   dV_w += P^T dO_i,  dK_w += dS^T Q_i       (wgmma RS: P^T / dS^T re-packed to 16 bit as the A operand,
@@ -54,12 +57,13 @@ struct BwdParams {
   float* dv_acc;
   int64_t dv_sb, dv_ss, dv_sh;
   int B, Sq, Sk, H;
+  int G;  // query heads per K/V head (grouped-query attention; 1 = MHA): K/V head hk serves heads hk*G .. hk*G+G-1
   float scale, scale_log2;
   int causal, causal_off;
-  const float* bias;  // optional additive bias per key [B|1, H, Sk] (fp32), or null
+  const float* bias;  // optional additive bias per key [B|1, H, Sk] (fp32, indexed by the query head), or null
   int64_t bias_sb, bias_sh;
   int* sem;     // deterministic mode: [B][H][nQ] turn counters ordering the dQ reductions by key block; else null
-  int* ticket;  // deterministic mode: [B][H] key-block tickets (a CTA's key block = the order in which it STARTED)
+  int* ticket;  // deterministic mode: [B][H/G] key-block tickets (a CTA's key block = the order in which it STARTED)
 };
 
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
@@ -112,23 +116,26 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
-  const int h = blockIdx.y, b = blockIdx.z;
+  const int hk = blockIdx.y, b = blockIdx.z;  // K/V head; its query heads are h0 .. h0 + G - 1
+  const int h0 = hk * p.G;
   // Key block of this CTA.  Deterministic mode orders the dQ reductions by key block and makes a CTA wait for
   // all lower key blocks; to make that wait deadlock-free without assuming anything about the order in which
   // the hardware dispatches blockIdx.x, the key block is a ticket drawn when the CTA starts: every lower
-  // ticket then belongs to a CTA that is already resident.
+  // ticket then belongs to a CTA that is already resident.  Tickets are per (batch, K/V head): the CTAs that
+  // share one are exactly the ones whose dQ reductions meet on the same (query head, Q block) turn counters.
   int kb = blockIdx.x;
   if (p.sem) {
-    if (threadIdx.x == 0) bars->key_block = atomicAdd(p.ticket + b * p.H + h, 1);
+    if (threadIdx.x == 0) bars->key_block = atomicAdd(p.ticket + b * (p.H / p.G) + hk, 1);
     __syncthreads();
     kb = bars->key_block;
   }
   const int k0 = kb * kBwdN;
   const int nQ = (p.Sq + kBwdM - 1) / kBwdM;
-  // first Q block that can see any key of this block: q >= k0 - off
+  // first Q block that can see any key of this block: q >= k0 - off (the same for every query head of the group)
   const int i_begin = p.causal ? max(0, k0 - p.causal_off) / kBwdM : 0;
   const int n_it = max(0, nQ - i_begin);
   if (n_it == 0) return;  // nothing visible: dK/dV contributions are zero (uniform exit, no barriers yet)
+  const int n_steps = p.G * n_it;  // step j: query head h0 + j / n_it, Q block i_begin + j % n_it
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -152,14 +159,15 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->kv_full, 2 * kBoxes * kBoxKV);
       for (int half = 0; half < kBoxes; ++half) {
-        tma_load_4d(smem + L::kOffK + half * kBoxKV, &tmK, &bars->kv_full, half * 64, h, k0, b);
-        tma_load_4d(smem + L::kOffV + half * kBoxKV, &tmV, &bars->kv_full, half * 64, h, k0, b);
+        tma_load_4d(smem + L::kOffK + half * kBoxKV, &tmK, &bars->kv_full, half * 64, hk, k0, b);
+        tma_load_4d(smem + L::kOffV + half * kBoxKV, &tmV, &bars->kv_full, half * 64, hk, k0, b);
       }
     }
-    for (int it = 0; it < n_it; ++it) {
+    int it = 0, h = h0;  // Q block (relative to i_begin) and query head of this step
+    for (int step = 0; step < n_steps; ++step) {
       const int q0 = (i_begin + it) * kBwdM;
-      const int st = it & 1;
-      mbar_wait(&bars->q_empty[st], ((it >> 1) & 1) ^ 1);
+      const int st = step & 1;
+      mbar_wait(&bars->q_empty[st], ((step >> 1) & 1) ^ 1);
       // row statistics of this Q block (lane handles rows lane, lane + 32): lse in log2 units, delta
       float* stat = sStat + st * 2 * kBwdM;
 #pragma unroll
@@ -183,6 +191,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         }
       }
       __syncwarp();
+      if (++it == n_it) it = 0, ++h;
     }
     return;
   }
@@ -196,13 +205,9 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int keys[2] = {k0 + kr_lo, k0 + kr_lo + 8};
   const float scale_log2 = p.scale_log2;
   // additive bias of this thread's keys, in log2 units (scores = q k^T scale + bias[key]; reference lao.py:155-173,
-  // "vector" bias): a per-row scalar in this key-row layout, folded into the exponent's FMA
+  // "vector" bias): a per-row scalar in this key-row layout, folded into the exponent's FMA; the bias is per query
+  // head, so it is (re)loaded at the first step of every head
   float bias2[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r)
-    bias2[r] = (p.bias && keys[r] < p.Sk)
-                   ? __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + keys[r]) * kBwdLog2e
-                   : 0.f;
   const bool reducer = kD == 128 || wg == 0;  // owns 64 columns of dQ
   const int n_red = kD == 128 ? 2 : 1;
 
@@ -214,12 +219,20 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const uint32_t kw = wg * 64 * 128;  // this group's 64 key rows inside every K / V box
   float* sDQ = reinterpret_cast<float*>(smem + L::kOffDQ) + wg * kBwdM * 64;
   mbar_wait(&bars->kv_full, 0);
-  for (int it = 0; it < n_it; ++it) {
+  int it = 0, h = h0;  // Q block (relative to i_begin) and query head of this step
+  for (int step = 0; step < n_steps; ++step) {
     const int q0 = (i_begin + it) * kBwdM;
-    const int st = it & 1;
+    const int st = step & 1;
     const uint32_t sQ = smem_u32(smem + L::kOffQ + st * kQStageB), sDO = smem_u32(smem + L::kOffDO + st * kQStageB);
     const float* stat = sStat + st * 2 * kBwdM;
-    mbar_wait(&bars->q_full[st], (it >> 1) & 1);
+    if (it == 0) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+        bias2[r] = (p.bias && keys[r] < p.Sk)
+                       ? __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + keys[r]) * kBwdLog2e
+                       : 0.f;
+    }
+    mbar_wait(&bars->q_full[st], (step >> 1) & 1);
 
     float s[32], dp[32];
     wgmma_fence();
@@ -282,8 +295,8 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     wgmma_commit();
 
     // dS^T -> smem [128 keys][64 q] (SW128: 16-byte chunk j of row r at j ^ (r % 8)), double-buffered: the buffer
-    // written here was last read by the dQ MMAs of block it - 2, which both warpgroups waited for before the
-    // barrier of block it - 1
+    // written here was last read by the dQ MMAs of step - 2, which both warpgroups waited for before the
+    // barrier of step - 1
     uint8_t* sDS = smem + L::kOffDS + st * kBwdN * 128;
 #pragma unroll
     for (int c = 0; c < 8; ++c)
@@ -327,9 +340,12 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       fence_proxy_async_smem();
       named_bar_sync(bar_id, 128);
       if (tid == 0) {
-        // deterministic mode: the fp32 adds into dq_acc[q block] happen in key-block order.  Key blocks that
-        // see a given Q block are 0..x_max and lower key blocks are tickets of CTAs that started earlier
-        // (see the top of the kernel), so waiting for our turn cannot deadlock.
+        // deterministic mode: the fp32 adds into dq_acc[query head, q block] happen in key-block order.  Key
+        // blocks that see a given Q block are 0..x_max (i_begin does not depend on the query head), and lower
+        // key blocks are tickets of CTAs of the same (batch, K/V head) that started earlier (see the top of the
+        // kernel).  A CTA visits every (query head, Q block) of its group once, in the same head-major order
+        // as every other CTA, and only ever waits for a lower ticket; by induction over tickets (ticket 0
+        // never waits) every wait ends, so waiting for our turn cannot deadlock.
         int* turn = p.sem ? p.sem + ((int64_t)b * p.H + h) * nQ + (i_begin + it) : nullptr;
         const int my_turn = kb * n_red + wg;
         if (turn) {
@@ -344,6 +360,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         }
       }
     }
+    if (++it == n_it) it = 0, ++h;
   }
   if (reducer && tid == 0) tma_store_wait<0>();
 
@@ -351,8 +368,8 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     if (keys[r] >= p.Sk) continue;
-    float* pk = p.dk_acc + (int64_t)b * p.dk_sb + (int64_t)keys[r] * p.dk_ss + (int64_t)h * p.dk_sh + 2 * t;
-    float* pv = p.dv_acc + (int64_t)b * p.dv_sb + (int64_t)keys[r] * p.dv_ss + (int64_t)h * p.dv_sh + 2 * t;
+    float* pk = p.dk_acc + (int64_t)b * p.dk_sb + (int64_t)keys[r] * p.dk_ss + (int64_t)hk * p.dk_sh + 2 * t;
+    float* pv = p.dv_acc + (int64_t)b * p.dv_sb + (int64_t)keys[r] * p.dv_ss + (int64_t)hk * p.dv_sh + 2 * t;
 #pragma unroll
     for (int c = 0; c < kD / 8; ++c) {
       float2 a = *reinterpret_cast<float2*>(pk + 8 * c);
@@ -373,7 +390,7 @@ static int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUte
   auto kern = bwd_chunk_kernel<kBF16, kD>;
   constexpr int smem = BwdLayout<kD>::kSmemBytes;
   BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sk + kBwdN - 1) / kBwdN, p.H, p.B);
+  dim3 grid((p.Sk + kBwdN - 1) / kBwdN, p.H / p.G, p.B);  // one CTA per (key block, K/V head, batch)
   kern<<<grid, kBwdThreads, smem, stream>>>(tmQ, tmK, tmV, tmDO, tmDQ, p);
   BA_CHECK_CUDA(cudaGetLastError());
   return BA_OK;
@@ -440,7 +457,16 @@ extern "C" int ba_bwd_chunk_bias(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
                                  ba_rowstat lse, ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc,
                                  ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int D, float scale, int mask_mode,
                                  int causal_offset, int flags, int dtype, void* stream) {
+  return ba_bwd_chunk_gqa(d_o, q, k, v, delta, lse, key_bias, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H, D, scale,
+                          mask_mode, causal_offset, flags, dtype, stream);
+}
+
+extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
+                                ba_rowstat lse, ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc,
+                                ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
+                                int mask_mode, int causal_offset, int flags, int dtype, void* stream) {
   using namespace ba;
+  BA_REQUIRE(H_kv > 0 && H % H_kv == 0, "ba_bwd_chunk: H_kv=%d must be positive and divide H=%d", H_kv, H);
   BA_REQUIRE(D == 128 || D == 64, "ba_bwd_chunk: head dim %d unsupported (64 or 128)", D);
   BA_REQUIRE(B > 0 && Sq > 0 && Sk > 0 && H > 0, "ba_bwd_chunk: empty problem B=%d Sq=%d Sk=%d H=%d", B, Sq, Sk, H);
   BA_REQUIRE(dtype == BA_DTYPE_FP16 || dtype == BA_DTYPE_BF16, "ba_bwd_chunk: bad dtype %d", dtype);
@@ -456,9 +482,9 @@ extern "C" int ba_bwd_chunk_bias(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
   int rc;
   if ((rc = make_tensor_map(&tmQ, q, B, Sq, H, D, dt, 2, 64, kBwdM, true))) return rc;
   if ((rc = make_tensor_map(&tmDO, d_o, B, Sq, H, D, dt, 2, 64, kBwdM, true))) return rc;
-  if ((rc = make_tensor_map(&tmK, k, B, Sk, H, D, dt, 2, 64, kBwdN, true))) return rc;
-  if ((rc = make_tensor_map(&tmV, v, B, Sk, H, D, dt, 2, 64, kBwdN, true))) return rc;
-  // dQ reductions: [64 rows][64 fp32 columns] boxes, no swizzle (one per reducing warpgroup)
+  if ((rc = make_tensor_map(&tmK, k, B, Sk, H_kv, D, dt, 2, 64, kBwdN, true))) return rc;
+  if ((rc = make_tensor_map(&tmV, v, B, Sk, H_kv, D, dt, 2, 64, kBwdN, true))) return rc;
+  // dQ reductions: [64 rows][64 fp32 columns] boxes, no swizzle (one per reducing warpgroup), H query heads
   if ((rc = make_tensor_map(&tmDQ, dq_acc, B, Sq, H, D, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 64, kBwdM, false)))
     return rc;
 
@@ -471,6 +497,7 @@ extern "C" int ba_bwd_chunk_bias(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
   p.dv_sb = dv_acc.stride_b, p.dv_ss = dv_acc.stride_s, p.dv_sh = dv_acc.stride_h;
   p.bias = key_bias.ptr, p.bias_sb = key_bias.stride_b, p.bias_sh = key_bias.stride_h;
   p.B = B, p.Sq = Sq, p.Sk = Sk, p.H = H;
+  p.G = H / H_kv;
   p.scale = scale;
   p.scale_log2 = scale * kBwdLog2e;
   p.causal = mask_mode == BA_MASK_CAUSAL;
@@ -478,8 +505,8 @@ extern "C" int ba_bwd_chunk_bias(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   p.sem = p.ticket = nullptr;
   if (flags & BA_BWD_DETERMINISTIC) {
-    const size_t n_turn = (size_t)B * H * ((Sq + kBwdM - 1) / kBwdM);
-    const size_t n = n_turn + (size_t)B * H;
+    const size_t n_turn = (size_t)B * H * ((Sq + kBwdM - 1) / kBwdM);  // per (batch, query head, Q block)
+    const size_t n = n_turn + (size_t)B * H_kv;                         // tickets per (batch, K/V head)
     p.sem = bwd_sem_workspace(n, st);
     if (p.sem) p.ticket = p.sem + n_turn;
     if (!p.sem) {

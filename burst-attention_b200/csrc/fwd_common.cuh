@@ -23,8 +23,9 @@ struct FwdParams {
   void* o_out;
   int64_t oout_sb, oout_ss, oout_sh;
   int B, Sq, Sk, H;
+  int G;              // query heads per K/V head (grouped-query attention; 1 = MHA): head h reads K/V head h / G
   float scale_log2;
-  const float* bias;  // optional additive bias per key [B|1, H, Sk] (fp32), or null
+  const float* bias;  // optional additive bias per key [B|1, H, Sk] (fp32, indexed by the query head), or null
   int64_t bias_sb, bias_sh;
   int causal;
   int causal_off;

@@ -7,6 +7,10 @@
 // prologue as the initial online-softmax state (m = lse, l = 1, acc = O) and the
 // merged state is written in the epilogue -- no separate merge pass over HBM.
 //
+// Grouped-query attention: K/V may have H / G heads; query head h reads K/V head h / G.  The grid is
+// (Q tiles, query heads, batch), so the G query heads of a group are adjacent in blockIdx.y and their CTAs sweep
+// the same K/V slice while it is resident in L2.
+//
 // Structure (one CTA = one 128-row Q tile of one (batch, head)):
 //   warpgroup 0   one TMA producer thread: Q once, then K_i / V_i tiles into 2-stage rings (and, with a key bias,
 //                 the tile's bias in log2 units); the other warps of the group only hand their registers over
@@ -109,6 +113,7 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     // ============================================================ TMA producer (warp 0)
     reg_alloc_dec<40>();
     if (warp != 0) return;
+    const int hk = h / p.G;  // K/V head of this query head
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->q_full, kTileBytes);
       for (int half = 0; half < kBoxes; ++half)
@@ -120,7 +125,7 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       if (lane == 0) {
         mbar_arrive_expect_tx(&bars->k_full[ks], kTileBytes);
         for (int half = 0; half < kBoxes; ++half)
-          tma_load_4d(sK + ks * kTileBytes + half * kBoxBytes, &tmK, &bars->k_full[ks], half * 64, h,
+          tma_load_4d(sK + ks * kTileBytes + half * kBoxBytes, &tmK, &bars->k_full[ks], half * 64, hk,
                       i * kBlockN, b);
       }
       if constexpr (kBias) {  // the stage's key bias in log2 units: lane handles keys lane + 32 j
@@ -139,7 +144,7 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         mbar_wait(&bars->v_empty[vs], vph ^ 1);
         mbar_arrive_expect_tx(&bars->v_full[vs], kTileBytes);
         for (int half = 0; half < kBoxes; ++half)
-          tma_load_4d(sV + vs * kTileBytes + half * kBoxBytes, &tmV, &bars->v_full[vs], half * 64, h,
+          tma_load_4d(sV + vs * kTileBytes + half * kBoxBytes, &tmV, &bars->v_full[vs], half * 64, hk,
                       i * kBlockN, b);
       }
       __syncwarp();
@@ -341,7 +346,15 @@ extern "C" int ba_fwd_chunk(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4
 extern "C" int ba_fwd_chunk_bias(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
                                  ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int D, float scale,
                                  int mask_mode, int causal_offset, int flags, int dtype, void* stream) {
+  return ba_fwd_chunk_gqa(q, k, v, key_bias, o_acc, lse, o_out, B, Sq, Sk, H, H, D, scale, mask_mode, causal_offset,
+                          flags, dtype, stream);
+}
+
+extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
+                                ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D,
+                                float scale, int mask_mode, int causal_offset, int flags, int dtype, void* stream) {
   using namespace ba;
+  BA_REQUIRE(H_kv > 0 && H % H_kv == 0, "ba_fwd_chunk: H_kv=%d must be positive and divide H=%d", H_kv, H);
   BA_REQUIRE(D == 128 || D == 64, "ba_fwd_chunk: head dim %d unsupported (64 or 128)", D);
   BA_REQUIRE(B > 0 && Sq > 0 && Sk > 0 && H > 0, "ba_fwd_chunk: empty problem B=%d Sq=%d Sk=%d H=%d", B, Sq, Sk, H);
   BA_REQUIRE(dtype == BA_DTYPE_FP16 || dtype == BA_DTYPE_BF16, "ba_fwd_chunk: bad dtype %d", dtype);
@@ -365,8 +378,8 @@ extern "C" int ba_fwd_chunk_bias(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
   const CUtensorMapDataType dt = lowp_dtype(dtype);
   int rc;
   if ((rc = make_tensor_map(&tmQ, q, B, Sq, H, D, dt, 2, 64, kBlockM, true))) return rc;
-  if ((rc = make_tensor_map(&tmK, k, B, Sk, H, D, dt, 2, 64, kBlockN, true))) return rc;
-  if ((rc = make_tensor_map(&tmV, v, B, Sk, H, D, dt, 2, 64, kBlockN, true))) return rc;
+  if ((rc = make_tensor_map(&tmK, k, B, Sk, H_kv, D, dt, 2, 64, kBlockN, true))) return rc;
+  if ((rc = make_tensor_map(&tmV, v, B, Sk, H_kv, D, dt, 2, 64, kBlockN, true))) return rc;
 
   FwdParams p;
   p.o_acc = static_cast<float*>(o_acc.ptr);
@@ -376,6 +389,7 @@ extern "C" int ba_fwd_chunk_bias(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
   p.o_out = o_out.ptr;
   p.oout_sb = o_out.stride_b, p.oout_ss = o_out.stride_s, p.oout_sh = o_out.stride_h;
   p.B = B, p.Sq = Sq, p.Sk = Sk, p.H = H;
+  p.G = H / H_kv;
   p.scale_log2 = scale * kLog2e;
   p.causal = mask_mode == BA_MASK_CAUSAL;
   p.causal_off = causal_offset;

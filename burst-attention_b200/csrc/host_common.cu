@@ -81,7 +81,7 @@ int make_tensor_map(CUtensorMap* out, const ba_tensor4& t, int B, int S, int H, 
 extern "C" const char* ba_selftest_last_error(void) { return ba::g_err; }
 #else
 extern "C" const char* ba_last_error(void) { return ba::g_err; }
-extern "C" int ba_version(void) { return 200; }
+extern "C" int ba_version(void) { return 201; }  // 201: grouped-query attention (ba_fwd_chunk_gqa, ba_bwd_chunk_gqa)
 extern "C" int ba_device_check(void) {
   int dev = 0;
   BA_CHECK_CUDA(cudaGetDevice(&dev));

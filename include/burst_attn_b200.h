@@ -89,6 +89,13 @@ int ba_fwd_chunk_bias(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_b
                       ba_tensor4 o_out, int B, int Sq, int Sk, int H, int D, float scale, int mask_mode,
                       int causal_offset, int flags, int dtype, void* stream);
 
+/* Grouped-query attention (GQA; MQA when H_kv == 1): the same as ba_fwd_chunk_bias with k, v of H_kv heads
+ * ([B,Sk,H_kv,D]).  Query head h attends with K/V head h / (H / H_kv); H % H_kv == 0 and H_kv > 0 are required.
+ * H applies to q, o_acc, o_out, lse and key_bias; H_kv to k and v.  H_kv == H is ba_fwd_chunk_bias.        */
+int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc, ba_rowstat lse,
+                     ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
+                     int causal_offset, int flags, int dtype, void* stream);
+
 /* delta[b,h,s] = sum_d O[b,s,h,d] * dO[b,s,h,d]  (burst_attn_interface.py:272-278) */
 int ba_bwd_delta(ba_tensor4 o, ba_tensor4 d_o, ba_rowstat delta, int B, int S, int H, int D, int dtype,
                  void* stream);
@@ -106,6 +113,14 @@ int ba_bwd_chunk(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
 int ba_bwd_chunk_bias(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
                       ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq, int Sk,
                       int H, int D, float scale, int mask_mode, int causal_offset, int flags, int dtype, void* stream);
+
+/* Grouped-query attention: the same as ba_bwd_chunk_bias with k, v, dk_acc, dv_acc of H_kv heads.  dK / dV of a
+ * K/V head accumulate the sum over its H / H_kv query heads.  H applies to q, d_o, delta, lse, key_bias and dq_acc.
+ * H % H_kv == 0 and H_kv > 0 are required; H_kv == H is ba_bwd_chunk_bias.                                      */
+int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
+                     ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq, int Sk,
+                     int H, int H_kv, int D, float scale, int mask_mode, int causal_offset, int flags, int dtype,
+                     void* stream);
 
 /* dst[b,s,h,d] (dtype) = src[b,s,h,d] (fp32); used once per backward to hand the
  * fp32 gradient accumulators back in the input dtype.                              */
