@@ -20,6 +20,12 @@
 //   dS^T -> smem (double-buffered), then dQ_i = dS K  (wgmma SS, both operands MN-major; head dim 128: each
 //   warpgroup computes 64 of the dQ columns, head dim 64: warpgroup 1 alone) -> smem -> cp.reduce.async.bulk.tensor
 //   (fp32 add in L2) into dq_acc.
+// Per step a consumer warpgroup keeps its own MMAs running under its element-wise work (five commit groups; four,
+// without dQ, for the non-reducing warpgroup at head dim 64):
+//   issue S^T | issue dP^T | wait<1>: P^T (exp2, bias, masks) + pack, under dP^T | wait<0> | issue dV |
+//   dS^T + pack + store to smem, under dV | barrier with the other warpgroup | issue dQ | issue dK |
+//   wait<1> (dV, dQ done): stage dQ + reduce-add, under dK | wait<0> | release the Q / dO stage.
+// The packed A operands (P^T for dV, dS^T for dK) stay untouched until the wait that retires their group.
 // smem (D = 128): K 32K, V 32K, Q 2x16K, dO 2x16K, dS^T 2x16K, dQ staging 16K per reducing warpgroup (single-
 // buffered: its next write waits for the previous reduce to have read it), row statistics 1K.
 #include <math.h>
@@ -234,6 +240,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     }
     mbar_wait(&bars->q_full[st], (step >> 1) & 1);
 
+    // S^T and dP^T as two commit groups: P^T is computed from S^T while dP^T is still running
     float s[32], dp[32];
     wgmma_fence();
 #pragma unroll
@@ -241,23 +248,23 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const uint32_t okv = (kk >> 2) * kBoxKV + kw + (kk & 3) * 32, oq = (kk >> 2) * kBoxQ + (kk & 3) * 32;
       wgmma_ss_n64<kBF16, 0, 0>(s, make_desc(sK + okv, 16, 1024), make_desc(sQ + oq, 16, 1024), kk > 0 ? 1u : 0u);
     }
+    wgmma_commit();
 #pragma unroll
     for (int kk = 0; kk < kD / 16; ++kk) {
       const uint32_t okv = (kk >> 2) * kBoxKV + kw + (kk & 3) * 32, oq = (kk >> 2) * kBoxQ + (kk & 3) * 32;
       wgmma_ss_n64<kBF16, 0, 0>(dp, make_desc(sV + okv, 16, 1024), make_desc(sDO + oq, 16, 1024), kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
-    wgmma_wait<0>();
+    wgmma_wait<1>();  // S^T done, dP^T may still run
     fence_regs<32>(s);
-    fence_regs<32>(dp);
 
+    // P^T in place of S^T (fp32, kept for dS^T) and packed to 16 bit as the A operand of dV.
     // visible iff key <= q + off  <=>  q >= key - off ; whole block visible when q0 + off >= k0 + 127
     const bool need_mask = p.causal && (q0 + p.causal_off < k0 + kBwdN - 1);
     uint32_t pp[16], ds[16];
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
       const float2 l2 = *reinterpret_cast<const float2*>(stat + 8 * c + 2 * t);
-      const float2 dl = *reinterpret_cast<const float2*>(stat + kBwdM + 8 * c + 2 * t);
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int e = 4 * c + 2 * r;
@@ -269,34 +276,40 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
           if (q < keys[r] - p.causal_off) p0 = 0.f;
           if (q + 1 < keys[r] - p.causal_off) p1 = 0.f;
         }
+        s[e] = p0, s[e + 1] = p1;
         pp[2 * c + r] = pack2<kBF16>(p0, p1);
-        ds[2 * c + r] = pack2<kBF16>(p0 * (dp[e] - dl.x), p1 * (dp[e + 1] - dl.y));
       }
     }
 
-    // dV += P^T dO, dK += dS^T Q   (B operands: [q rows][d] tiles read MN-major)
+    // dV += P^T dO   (B operand: [q rows][d] tile read MN-major); pp is read by the MMA until the wait<1> below
+    wgmma_wait<0>();  // dP^T done
+    fence_regs<32>(dp);
     fence_regs<16>(pp);
-    fence_regs<16>(ds);
     fence_regs<kAcc>(dv);
-    fence_regs<kAcc>(dk);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kBwdM / 16; ++kk) {
       const uint64_t d_do = make_desc(sDO + kk * 16 * 128, kBoxQ, 1024);
-      const uint64_t d_q = make_desc(sQ + kk * 16 * 128, kBoxQ, 1024);
-      if constexpr (kD == 128) {
-        wgmma_rs_n128<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
-        wgmma_rs_n128<kBF16, 1>(dk, ds + 4 * kk, d_q, 1u);
-      } else {
-        wgmma_rs_n64<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
-        wgmma_rs_n64<kBF16, 1>(dk, ds + 4 * kk, d_q, 1u);
-      }
+      if constexpr (kD == 128) wgmma_rs_n128<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
+      else wgmma_rs_n64<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
     }
     wgmma_commit();
 
+    // dS^T = P^T o (dP^T - delta) while dV runs
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const float2 dl = *reinterpret_cast<const float2*>(stat + kBwdM + 8 * c + 2 * t);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int e = 4 * c + 2 * r;
+        ds[2 * c + r] = pack2<kBF16>(s[e] * (dp[e] - dl.x), s[e + 1] * (dp[e + 1] - dl.y));
+      }
+    }
+
     // dS^T -> smem [128 keys][64 q] (SW128: 16-byte chunk j of row r at j ^ (r % 8)), double-buffered: the buffer
-    // written here was last read by the dQ MMAs of step - 2, which both warpgroups waited for before the
-    // barrier of step - 1
+    // written here was last read by the dQ MMAs of step - 2.  Each reducing warpgroup's wgmma_wait<1> of step - 2
+    // completes its dQ group (dV and dQ are the two oldest of its three groups), and that wait comes before the
+    // warpgroup reaches the barrier of step - 1, which this warpgroup has passed.
     uint8_t* sDS = smem + L::kOffDS + st * kBwdN * 128;
 #pragma unroll
     for (int c = 0; c < 8; ++c)
@@ -308,8 +321,22 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     fence_proxy_async_smem();
     named_bar_sync(1, 256);
 
-    // dQ[:, 64 wg .. 64 wg + 63] = dS K  (A = dS^T tile read MN-major, B = K tile read MN-major)
+    // dQ[:, 64 wg .. 64 wg + 63] = dS K  (A = dS^T tile read MN-major, B = K tile read MN-major), then
+    // dK += dS^T Q (B operand read MN-major) as the last group: it runs on under the dQ staging below
+    // (head dim 64: the non-reducing warpgroup issues dK alone; each role runs its whole issue-to-wait sequence in
+    // one branch, so that no wgmma group crosses a divergent path, which would make ptxas serialize them)
     float dq[32];
+    fence_regs<16>(ds);
+    fence_regs<kAcc>(dk);
+    auto issue_dk = [&]() {
+#pragma unroll
+      for (int kk = 0; kk < kBwdM / 16; ++kk) {
+        const uint64_t d_q = make_desc(sQ + kk * 16 * 128, kBoxQ, 1024);
+        if constexpr (kD == 128) wgmma_rs_n128<kBF16, 1>(dk, ds + 4 * kk, d_q, 1u);
+        else wgmma_rs_n64<kBF16, 1>(dk, ds + 4 * kk, d_q, 1u);
+      }
+      wgmma_commit();
+    };
     if (reducer) {
       const uint32_t a0 = smem_u32(sDS), b0 = sK + wg * kBoxKV;
       wgmma_fence();
@@ -318,13 +345,15 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         wgmma_ss_n64<kBF16, 1, 1>(dq, make_desc(a0 + kk * 16 * 128, 8192, 1024),
                                   make_desc(b0 + kk * 16 * 128, kBoxKV, 1024), kk > 0 ? 1u : 0u);
       wgmma_commit();
+      issue_dk();
+      wgmma_wait<1>();  // dV and dQ done, dK may still run
+    } else {
+      wgmma_fence();
+      issue_dk();
+      wgmma_wait<1>();  // dV done, dK may still run
     }
-    wgmma_wait<0>();
     fence_regs<kAcc>(dv);
-    fence_regs<kAcc>(dk);
-    // Q, dO and the statistics of this stage are no longer read by this warp
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars->q_empty[st]);
+    fence_regs<16>(pp);
 
     if (reducer) {
       fence_regs<32>(dq);
@@ -360,6 +389,12 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         }
       }
     }
+    wgmma_wait<0>();  // dK done: ds may be rewritten, and Q of this stage is no longer read
+    fence_regs<kAcc>(dk);
+    fence_regs<16>(ds);
+    // Q, dO and the statistics of this stage are no longer read by this warp
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->q_empty[st]);
     if (++it == n_it) it = 0, ++h;
   }
   if (reducer && tid == 0) tma_store_wait<0>();

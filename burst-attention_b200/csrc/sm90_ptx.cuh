@@ -62,7 +62,10 @@ BA_DEVICE bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug traps after ~30 s (-> CUDA error surfaced to the
-// host) instead of hanging the GPU box.
+// host at its next synchronize) instead of hanging the GPU.  The watchdog must
+// make no function call: a call (printf -> vprintf) inside a kernel that issues
+// wgmma makes ptxas serialize every wgmma of that kernel (warning C7510), which
+// the build refuses.  To locate a fault, add a printf here while debugging.
 BA_DEVICE uint64_t global_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -82,8 +85,6 @@ BA_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) {
       if (mbar_try_wait(bar, parity)) return;
     if (global_ns() - t0 > 30000000000ull) break;
   }
-  printf("ba: mbarrier watchdog block(%d,%d,%d) thread %d bar@%u parity %u\n", blockIdx.x, blockIdx.y,
-         blockIdx.z, threadIdx.x, smem_u32(bar), parity);
   __trap();
 #endif
 }
