@@ -6,7 +6,9 @@ What is the same as the reference: names, argument order and defaults, shard
 layouts (contiguous / zigzag halves / striped, test/test_burst.py:44-58), the
 ring schedules (forward: K/V rotate, :214-242; backward: the Q-bundle
 (delta, dO, Q, lse) rotates and the partial dQ rides one hop behind it,
-:291-396), output dtype, the assertion that causal needs flash == "cuda".
+:291-396), output dtype, the assertion that causal needs flash == "cuda".  The hierarchical ("double")
+ring (reference comm.py:187-254) runs through the same two drivers (``_ring_forward`` / ``_bwd_rounds``):
+the flat ring is its special case of one node.
 
 What is H100-native instead (DESIGN.md): every round is ONE kernel launch of the
 C-ABI library (carried (O, lse) state and fp32 dQ/dK/dV accumulation fused into
@@ -94,6 +96,15 @@ class _Topology:
             return (self.rank - (r - 1)) % self.W
         return get_partition_id([self.intra, self.inter], r)
 
+    def rings(self):
+        """(ring, inter, inter_dq): the ring the blocks hop round inside a cycle, and on the hierarchical ring the
+        inter-node rings of the block prefetch and of the dQ node sums (None on the flat ring)."""
+        if not self.hier:
+            return Ring(self.group, tag="ring"), None, None
+        # the copy-engine transport serves the flat ring only: its receive buffers are tied to one ring's arena
+        return (Ring(self.intra, tag="ring", transport="nccl"), Ring(self.inter, tag="inter", transport="nccl"),
+                Ring(self.inter_dq if self.inter_dq is not None else self.inter, tag="inter_dq", transport="nccl"))
+
 
 def split2_gethalf(inp, first_dim, half_idx=0):
     """Half-sequence VIEW (reference :96-106); never copied here."""
@@ -130,14 +141,23 @@ def _fwd_round(ops, q, k, v, o_acc, lse, out, scale, causal, off, first, last, s
     """One forward ring round, split over K/V blocks that fit L2 (each block is one kernel launch with
     the carried state; the state pass costs 2 x 512 B per row and head, the block > 8 MB of math)."""
     blk = _l2_block()
-    Sq, Sk = q.shape[seq_dim], k.shape[seq_dim]
-    if Sk <= blk + blk // 2:
+    if k.shape[seq_dim] <= blk + blk // 2:
         ops.fwd_chunk(q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, **_bias_kw(bias))
         return
+    _fwd_blocks(ops, q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, blk, bias)
+
+
+def _fwd_blocks(ops, q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, blk, bias=None,
+                before=None):
+    """A forward round as one launch per block of ``blk`` keys; ``before(c)``, if given, runs first in the step
+    of block c (host_stream.py waits there for the block's upload)."""
+    Sq, Sk = q.shape[seq_dim], k.shape[seq_dim]
     n = (Sk + blk - 1) // blk
     for c in range(n):
         c0 = c * blk
         kc, vc = k.narrow(seq_dim, c0, min(blk, Sk - c0)), v.narrow(seq_dim, c0, min(blk, Sk - c0))
+        if before is not None:
+            before(c)
         if not causal:
             ops.fwd_chunk(q, kc, vc, o_acc, lse, out, scale, False, 0, first and c == 0, last and c == n - 1, seq_dim,
                           **_bias_kw(bias, c0, min(blk, Sk - c0)))
@@ -164,24 +184,30 @@ def _bwd_round(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, caus
                bias=None):
     """One backward ring round, split over blocks of Q-bundle rows that fit L2."""
     blk = _l2_block()
-    Sq, Sk = q.shape[seq_dim], k.shape[seq_dim]
+    Sq = q.shape[seq_dim]
     if Sq <= blk + blk // 2:
         ops.bwd_chunk(g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
                       **_bias_kw(bias))
         return
     for r0 in range(0, Sq, blk):
-        n = min(blk, Sq - r0)
-        kk, vv, dk, dv, o2, bkw = k, v, dk_acc, dv_acc, off, _bias_kw(bias)
-        if causal:
-            kmax = min(Sk, r0 + n + off)  # keys visible to the last row of this block
-            if kmax <= 0:
-                continue
-            kk, vv, bkw = k.narrow(seq_dim, 0, kmax), v.narrow(seq_dim, 0, kmax), _bias_kw(bias, 0, kmax)
-            dk, dv = dk_acc.narrow(seq_dim, 0, kmax), dv_acc.narrow(seq_dim, 0, kmax)
-            o2 = off + r0
-        ops.bwd_chunk(g.narrow(seq_dim, r0, n), q.narrow(seq_dim, r0, n), kk, vv, delta.narrow(2, r0, n),
-                      lse.narrow(2, r0, n), dq_part.narrow(seq_dim, r0, n), dk, dv, scale, causal, o2, seq_dim,
-                      deterministic, **bkw)
+        _bwd_rows(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
+                  r0, min(blk, Sq - r0), bias)
+
+
+def _bwd_rows(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
+              r0, n, bias=None):
+    """Rows [r0, r0+n) of a backward round as one launch over the keys they see (none: no launch)."""
+    kk, vv, dk, dv, o2, bkw = k, v, dk_acc, dv_acc, off, _bias_kw(bias)
+    if causal:
+        kmax = min(k.shape[seq_dim], r0 + n + off)  # keys visible to the last row of this block
+        if kmax <= 0:
+            return
+        kk, vv, bkw = k.narrow(seq_dim, 0, kmax), v.narrow(seq_dim, 0, kmax), _bias_kw(bias, 0, kmax)
+        dk, dv = dk_acc.narrow(seq_dim, 0, kmax), dv_acc.narrow(seq_dim, 0, kmax)
+        o2 = off + r0
+    ops.bwd_chunk(g.narrow(seq_dim, r0, n), q.narrow(seq_dim, r0, n), kk, vv, delta.narrow(2, r0, n),
+                  lse.narrow(2, r0, n), dq_part.narrow(seq_dim, r0, n), dk, dv, scale, causal, o2, seq_dim,
+                  deterministic, **bkw)
 
 
 def _check_inputs(q, k, v, seq_dim):
@@ -220,12 +246,17 @@ def _fwd_dispatch(ops, mode, r, W, i, j, q, cur_k, cur_v, o_acc, lse, out, scale
 # forward ring (reference OpBurstAttn.forward :171-253, OpBurstAttnStrip.forward :411-493)
 # --------------------------------------------------------------------------- #
 def _ring_forward(q, k, v, scale, seq_dim, mode, topo):
-    """mode: "none" (non-causal) | "zigzag" | "striped".  Returns (out, lse[B,H,S] fp32)."""
-    if topo.hier:
-        return _ring_forward_hier(q, k, v, scale, seq_dim, mode, topo)
+    """mode: "none" (non-causal) | "zigzag" | "striped".  Returns (out, lse[B,H,S] fp32).
+
+    Rounds run in M cycles of L steps (the flat ring is one cycle, L = W).  Within a cycle K/V hop round the
+    intra-node ring; on the hierarchical ring (reference comm.py:187-254, SURVEY.md Appendix C) the block a
+    cycle starts with is at the same time forwarded to the next node over the inter-node ring, where it starts
+    the following cycle -- a prefetch with L rounds of kernel time to hide behind.  Unlike the reference no
+    send-side copy is made: the cycle's starting block is never a receive target while it is in flight (two
+    inter-node buffers alternate)."""
     ops = get_ops()
-    ring = Ring(topo.group, tag="ring")
-    W, i = ring.world_size, ring.rank
+    ring, inter, _ = topo.rings()
+    L, M, W, i = topo.L, topo.M, topo.W, topo.rank
     B, S, H = q.shape[0], q.shape[seq_dim], q.shape[3 - seq_dim]
     if mode == "zigzag":
         assert S % 2 == 0, "zigzag causal sharding needs an even local sequence length"
@@ -235,58 +266,26 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo):
     o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device) if need_state else None
     if W > 1:
         k, v = k.contiguous(), v.contiguous()
-    ring.begin(q, [_nbytes(k), _nbytes(v)] * min(2, W - 1))
-    recv = [[ring.empty_like(k), ring.empty_like(v)] for _ in range(min(2, W - 1))]
-    cur_k, cur_v = k, v
-    for r in range(1, W + 1):
-        j = topo.source(r)  # source rank of the held K/V (App. B)
-        with _Range(f"fwd_round_{r}"):
-            if r != W:
-                nxt = recv[(r - 1) % len(recv)]
-                ring.post([cur_k, cur_v], nxt)
-            _fwd_dispatch(ops, mode, r, W, i, j, q, cur_k, cur_v, o_acc, lse, out, scale, seq_dim)
-            if r != W:
-                ring.wait()
-                cur_k, cur_v = nxt
-    return out, lse
-
-
-def _ring_forward_hier(q, k, v, scale, seq_dim, mode, topo):
-    """Hierarchical ("double") ring, W = L*M (reference comm.py:187-254, SURVEY.md Appendix C): rounds run
-    in M cycles of L steps.  Within a cycle K/V hop round the intra-node ring; the block a cycle starts
-    with is at the same time forwarded to the next node over the inter-node ring, where it starts the
-    following cycle -- a prefetch with L rounds of kernel time to hide behind.  Unlike the reference no
-    send-side copy is made: the cycle's starting block is never a receive target while it is in flight
-    (two inter-node buffers alternate)."""
-    ops = get_ops()
-    # (the copy-engine transport serves the flat ring only: its receive buffers are tied to one ring's arena)
-    intra, inter = Ring(topo.intra, tag="ring", transport="nccl"), Ring(topo.inter, tag="inter", transport="nccl")
-    L, M, W, i = topo.L, topo.M, topo.W, topo.rank
-    B, S, H = q.shape[0], q.shape[seq_dim], q.shape[3 - seq_dim]
-    if mode == "zigzag":
-        assert S % 2 == 0, "zigzag causal sharding needs an even local sequence length"
-    out = torch.empty_like(q)
-    lse = torch.empty((B, H, S), dtype=torch.float32, device=q.device)
-    o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device)
-    k, v = k.contiguous(), v.contiguous()
-    recv = [[torch.empty_like(k), torch.empty_like(v)] for _ in range(min(2, L - 1))]
+    ring.begin(q, [_nbytes(k), _nbytes(v)] * min(2, L - 1))
+    recv = [[ring.empty_like(k), ring.empty_like(v)] for _ in range(min(2, L - 1))]
     xbuf = [[torch.empty_like(k), torch.empty_like(v)] for _ in range(min(2, M - 1))]
     cur = [k, v]
     for r in range(1, W + 1):
         c, t = divmod(r - 1, L)
-        j = topo.source(r)
-        if t == 0 and c != M - 1:  # next cycle's starting block, from the previous node
-            inter.post(cur, xbuf[c % len(xbuf)])
-        if t != L - 1:
-            nxt = recv[(r - 1) % len(recv)]
-            intra.post(cur, nxt)
-        _fwd_dispatch(ops, mode, r, W, i, j, q, cur[0], cur[1], o_acc, lse, out, scale, seq_dim)
-        if t != L - 1:
-            intra.wait()
-            cur = nxt
-        elif c != M - 1:
-            inter.wait()
-            cur = xbuf[c % len(xbuf)]
+        j = topo.source(r)  # source rank of the held K/V (App. B)
+        with _Range(f"fwd_round_{r}"):
+            if t == 0 and c != M - 1:  # next cycle's starting block, from the previous node
+                inter.post(cur, xbuf[c % len(xbuf)])
+            if t != L - 1:
+                nxt = recv[(r - 1) % len(recv)]
+                ring.post(cur, nxt)
+            _fwd_dispatch(ops, mode, r, W, i, j, q, cur[0], cur[1], o_acc, lse, out, scale, seq_dim)
+            if t != L - 1:
+                ring.wait()
+                cur = nxt
+            elif c != M - 1:
+                inter.wait()
+                cur = xbuf[c % len(xbuf)]
     return out, lse
 
 
@@ -336,57 +335,11 @@ def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, determini
         _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, scale, seq_dim, deterministic)
 
     bundle = [delta, d_o, q, lse.contiguous()]
-    # `part`: this round's dQ partial (the kernel reduce-adds into it)
     if W == 1:
-        part = torch.zeros(q.shape, **f32)
-        round_kernel(1, i, bundle, part)
-        dq_final = part
-    elif topo.hier:
-        part = torch.zeros(q.shape, **f32)
-        dq_final = _bwd_rounds_hier(ops, topo, round_kernel, bundle, part, q.shape, f32, seq_dim)
+        dq_final = torch.zeros(q.shape, **f32)
+        round_kernel(1, i, bundle, dq_final)
     else:
-        ring = Ring(topo.group, tag="ring")
-        # every buffer that is ever the destination of a hop comes from the ring (the copy-engine transport
-        # keeps them in its IPC-mapped arena): two bundle sets and the three rotating fp32 dQ buffers
-        ring.begin(q, [_nbytes(t) for t in bundle] * min(2, W - 1) + [4 * q.numel()] * 3)
-        recv = [[ring.empty_like(t) for t in bundle] for _ in range(min(2, W - 1))]
-        hold = None                      # fp32 dQ accumulated for the bundle held in the previous round
-        part = ring.empty(q.shape, torch.float32, dev)
-        part.zero_()
-        spare = [ring.empty(q.shape, torch.float32, dev), ring.empty(q.shape, torch.float32, dev)]
-        for r in range(1, W + 1):
-            j = topo.source(r)
-            srcs: List[torch.Tensor] = []
-            dsts: List[torch.Tensor] = []
-            if r != W:  # bundle hop (:295-299)
-                nxt = recv[(r - 1) % len(recv)]
-                srcs += bundle
-                dsts += nxt
-            if r != 1:  # dQ hop, one behind its bundle (:300-302)
-                inbound = spare.pop()
-                srcs.append(hold)
-                dsts.append(inbound)
-            with _Range(f"bwd_round_{r}"):
-                if srcs:
-                    ring.post(srcs, dsts)
-                round_kernel(r, j, bundle, part)
-                if srcs:
-                    ring.wait()
-            if r != W:
-                bundle = nxt
-            if r == 1:
-                hold, part = part, spare.pop()
-                part.zero_()
-            else:
-                ops.accumulate(part, inbound, seq_dim)  # dq += buf (:379-390), in fp32
-                spare.append(hold)
-                hold = inbound
-                if r != W:
-                    part.zero_()
-        # final hop home (:393-396)
-        dq_final = spare.pop()
-        ring.post([hold], [dq_final])
-        ring.wait()
+        dq_final = _bwd_rounds(ops, topo, round_kernel, bundle, q, seq_dim)
 
     dq = torch.empty_like(q)
     dk = torch.empty_like(k)
@@ -397,29 +350,36 @@ def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, determini
     return dq, dk, dv
 
 
-def _bwd_rounds_hier(ops, topo, round_kernel, bundle, part, qshape, f32, seq_dim):
-    """Backward rounds over the hierarchical ring (W = L*M); returns the fp32 dQ of this rank's own rows.
+def _bwd_rounds(ops, topo, round_kernel, bundle, q, seq_dim):
+    """Backward rounds over the ring (W > 1, M cycles of L steps as in the forward); returns the fp32 dQ of
+    this rank's own rows.
 
-    The Q-bundle travels exactly like K/V in the forward (intra-node hops inside a cycle, the cycle's
-    starting bundle prefetched to the next node).  Its dQ comes home in two levels (the reference's
-    ``double_ring_send_recv_q``, comm.py:187-213, restated):
-      * inside a cycle the partial rides one intra-node hop behind its bundle and picks up each rank's
-        contribution (as in the flat ring); one more intra-node hop after the cycle's last step closes the
-        ring, so the NODE sum for a bundle lands on the rank that started it in this node;
-      * node sums chain along the inter-node ring: at the start of cycle c the node sum of the bundle
-        started in cycle c-1 is added to the running sum received from the previous node and sent on --
-        L rounds of kernel time to hide behind.  After the last cycle the same step is the hop home.
+    The Q-bundle travels exactly like K/V in the forward (hops inside a cycle; on the hierarchical ring the
+    cycle's starting bundle is prefetched to the next node).  Its dQ comes home in two levels (the
+    reference's ``double_ring_send_recv_q``, comm.py:187-213, restated):
+      * inside a cycle the partial rides one hop behind its bundle (:300-302) and picks up each rank's
+        contribution; one more hop after the cycle's last step closes the ring, so the NODE sum for a bundle
+        lands on the rank that started it in this node -- on the flat ring that is the hop home (:393-396);
+      * on the hierarchical ring node sums chain along the inter-node ring: at the start of cycle c the node
+        sum of the bundle started in cycle c-1 is added to the running sum received from the previous node
+        and sent on -- L rounds of kernel time to hide behind.  After the last cycle the same step is the hop
+        home.
     """
     L, M, W = topo.L, topo.M, topo.W
-    intra = Ring(topo.intra, tag="ring", transport="nccl")
-    inter = Ring(topo.inter, tag="inter", transport="nccl")
-    inter_q = Ring(topo.inter_dq if topo.inter_dq is not None else topo.inter, tag="inter_dq", transport="nccl")
-    recv = [[torch.empty_like(t) for t in bundle] for _ in range(min(2, L - 1))]
+    ring, inter, inter_q = topo.rings()
+    dev = q.device
+    # every buffer that is ever the destination of a hop on `ring` comes from it (the copy-engine transport
+    # keeps them in its IPC-mapped arena): two bundle sets and the three rotating fp32 dQ buffers, all the
+    # flat ring ever takes; only the hierarchical ring's node-sum chain takes more
+    ring.begin(q, [_nbytes(t) for t in bundle] * min(2, L - 1) + [4 * q.numel()] * 3)
+    recv = [[ring.empty_like(t) for t in bundle] for _ in range(min(2, L - 1))]
     xbuf = [[torch.empty_like(t) for t in bundle] for _ in range(min(2, M - 1))]
-    free: List[torch.Tensor] = []
+    part = ring.empty(q.shape, torch.float32, dev)  # this round's dQ partial (the kernel reduce-adds into it)
+    part.zero_()
+    free = [ring.empty(q.shape, torch.float32, dev), ring.empty(q.shape, torch.float32, dev)]
 
     def take():
-        return free.pop() if free else torch.empty(qshape, **f32)
+        return free.pop() if free else ring.empty(q.shape, torch.float32, dev)
 
     hold = None      # dQ accumulated in this node for the bundle held in the previous round
     running = None   # inter-node running sum in flight to the next node (kept alive until awaited)
@@ -440,8 +400,7 @@ def _bwd_rounds_hier(ops, topo, round_kernel, bundle, part, qshape, f32, seq_dim
         j = topo.source(r)
         srcs: List[torch.Tensor] = []
         dsts: List[torch.Tensor] = []
-        inbound = None
-        if t != L - 1:  # bundle hop inside the node
+        if t != L - 1:  # bundle hop (:295-299)
             nxt = recv[(r - 1) % len(recv)]
             srcs += bundle
             dsts += nxt
@@ -449,13 +408,14 @@ def _bwd_rounds_hier(ops, topo, round_kernel, bundle, part, qshape, f32, seq_dim
             inbound = take()
             srcs.append(hold)
             dsts.append(inbound)
-        if srcs:
-            intra.post(srcs, dsts)
-        if t == 0 and c != M - 1:  # next cycle's starting bundle, from the previous node
-            inter.post(bundle, xbuf[c % len(xbuf)])
-        round_kernel(r, j, bundle, part)
-        if srcs:
-            intra.wait()
+        with _Range(f"bwd_round_{r}"):
+            if srcs:
+                ring.post(srcs, dsts)
+            if t == 0 and c != M - 1:  # next cycle's starting bundle, from the previous node
+                inter.post(bundle, xbuf[c % len(xbuf)])
+            round_kernel(r, j, bundle, part)
+            if srcs:
+                ring.wait()
         if t == 0:
             if r != 1:
                 free.append(hold)
@@ -463,7 +423,7 @@ def _bwd_rounds_hier(ops, topo, round_kernel, bundle, part, qshape, f32, seq_dim
             hold, part = part, take()
             part.zero_()
         else:
-            ops.accumulate(part, inbound, seq_dim)
+            ops.accumulate(part, inbound, seq_dim)  # dq += buf (:379-390), in fp32
             free.append(hold)
             hold = inbound
             if r != W:
@@ -473,13 +433,15 @@ def _bwd_rounds_hier(ops, topo, round_kernel, bundle, part, qshape, f32, seq_dim
         elif c != M - 1:
             inter.wait()
             bundle = xbuf[c % len(xbuf)]
-    # close the last cycle's intra-node ring, then the last inter-node hop is the hop home (:393-396)
-    node_sum = take()
-    intra.post([hold], [node_sum])
-    intra.wait()
-    chain(node_sum)
-    inter_q.wait()
-    return inter_in
+    # close the last cycle's ring; on the hierarchical ring the last inter-node hop is then the hop home
+    home = take()
+    ring.post([hold], [home])
+    ring.wait()
+    if M > 1:
+        chain(home)
+        inter_q.wait()
+        home = inter_in
+    return home
 
 
 # --------------------------------------------------------------------------- #

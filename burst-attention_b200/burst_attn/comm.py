@@ -23,7 +23,7 @@ A ``Ring`` here is always ONE ring over ONE group.  The reference's intra/inter
 "double ring" (comm.py:187-254) is composed by the drivers from up to three of
 them -- intra-node hops, inter-node prefetch of the block that starts the next
 cycle, inter-node chain of the dQ node sums (burst_attn_interface.py:
-``_ring_forward_hier`` / ``_bwd_rounds_hier``) -- so each level has its own
+``_ring_forward`` / ``_bwd_rounds``) -- so each level has its own
 communicator and side stream and is awaited independently.  8 GPUs on one
 NVSwitch are a uniform fabric where the flat ring is as good; the hierarchy is for
 W spanning several NVLink domains.

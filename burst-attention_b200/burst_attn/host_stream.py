@@ -21,6 +21,7 @@ from __future__ import annotations
 
 import torch
 
+from .burst_attn_interface import _bwd_rows, _fwd_blocks
 from .chunk_ops import get_ops
 
 _streams = {}
@@ -73,21 +74,8 @@ def forward(q, k, v, scale, seq_dim, causal, blk):
             ev.append(e)
     for t in (qd, kd, vd):
         t.record_stream(up)
-    off = 0
-    for c, (c0, cn) in enumerate(kblocks):
-        cur.wait_event(ev[c])
-        kc, vc = kd.narrow(seq_dim, c0, cn), vd.narrow(seq_dim, c0, cn)
-        first, last = c == 0, c == n - 1
-        if not causal:
-            ops.fwd_chunk(qd, kc, vc, o_acc, lse, out, scale, False, 0, first, last, seq_dim)
-            continue
-        r_start = max(0, (c0 - off) // 256 * 256)  # rows before it see none of this block's keys
-        if r_start >= S:
-            break
-        ops.fwd_chunk(qd.narrow(seq_dim, r_start, S - r_start), kc, vc, o_acc.narrow(seq_dim, r_start, S - r_start),
-                      lse.narrow(2, r_start, S - r_start), None, scale, True, r_start + off - c0, first, False, seq_dim)
-    if causal:
-        ops.cast(o_acc, out, seq_dim)
+    _fwd_blocks(ops, qd, kd, vd, o_acc, lse, out, scale, causal, 0, True, True, seq_dim, blk,
+                before=lambda c: cur.wait_event(ev[c]))
     o_host = _pinned_like(q.shape, q.dtype)
     done = torch.cuda.Event()
     done.record(cur)
@@ -137,28 +125,23 @@ def backward(d_o, saved, scale, seq_dim, causal, blk, deterministic):
             down.wait_event(e)
             host.narrow(seq_dim, s0, sn).copy_(lowp.narrow(seq_dim, s0, sn), non_blocking=True)
 
-    off = 0
     for i, (r0, rn) in enumerate(rblocks):
         cur.wait_event(ev[i])
         gb, qb = g.narrow(seq_dim, r0, rn), qd.narrow(seq_dim, r0, rn)
         db, lb = delta.narrow(2, r0, rn), lse.narrow(2, r0, rn)
         ops.delta(out.narrow(seq_dim, r0, rn), gb, db, seq_dim)
         dqb = dq_acc.narrow(seq_dim, r0, rn)
-        last_rows = i == len(rblocks) - 1
-        if not last_rows:
-            kmax = min(Sk, r0 + rn + off) if causal else Sk  # keys visible to the last row of this block
-            if kmax > 0:
-                ops.bwd_chunk(gb, qb, kd.narrow(seq_dim, 0, kmax), vd.narrow(seq_dim, 0, kmax), db, lb, dqb,
-                              dk_acc.narrow(seq_dim, 0, kmax), dv_acc.narrow(seq_dim, 0, kmax), scale, causal,
-                              off + r0, seq_dim, deterministic)
+        if i < len(rblocks) - 1:
+            _bwd_rows(ops, g, qd, kd, vd, delta, lse, dq_acc, dk_acc, dv_acc, scale, causal, 0, seq_dim, deterministic,
+                      r0, rn)
             ship(dq_acc, dq16, dq_h, r0, rn)
             continue
         # last row block: one launch per key block, so every dK / dV block is final right after its launch
         for k0, kn in kblocks:
-            if not causal or k0 <= r0 + rn - 1 + off:
+            if not causal or k0 <= r0 + rn - 1:
                 ops.bwd_chunk(gb, qb, kd.narrow(seq_dim, k0, kn), vd.narrow(seq_dim, k0, kn), db, lb, dqb,
                               dk_acc.narrow(seq_dim, k0, kn), dv_acc.narrow(seq_dim, k0, kn), scale, causal,
-                              off + r0 - k0, seq_dim, deterministic)
+                              r0 - k0, seq_dim, deterministic)
             ship(dk_acc, dk16, dk_h, k0, kn)
             ship(dv_acc, dv16, dv_h, k0, kn)
         ship(dq_acc, dq16, dq_h, r0, rn)

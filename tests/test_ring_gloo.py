@@ -1,9 +1,12 @@
-"""World-size 2 and 4 CPU tests (gloo) of the N>1 path: the ring drivers behind
+"""World-size 2 to 8 CPU tests (gloo) of the N>1 path: the ring drivers behind
 burst_attn_func / burst_attn_func_striped -- K/V rotation, the Q-bundle + dQ
-ring of the backward, zigzag / striped shard views -- run with the oracle-backed
-chunk operators injected (tests only) and are compared, through autograd, with
-dense attention on the full sequence (the reference's protocol,
-test/test_burst.py:159-219)."""
+ring of the backward, zigzag / striped shard views, the hierarchical ring --
+run with the oracle-backed chunk operators injected (tests only) and are
+compared, through autograd, with dense attention on the full sequence (the
+reference's protocol, test/test_burst.py:159-219).  With grouped-query K/V
+(fewer heads than Q) the reference is dense attention on K/V expanded per
+group, and each forward hop must carry 1/G of the bytes of the same call with
+MHA K/V."""
 import os
 import socket
 import sys
@@ -66,7 +69,97 @@ def _install_deferred_transport():
     comm.Ring.wait = wait
 
 
-def _worker(rank, world, port, case, seq_dim, errq, intra=0, dq_groups=False):
+HQ = 4
+HKV_CASES = (2, 1)  # grouped-query K/V: G = 2 (GQA) and G = Hq (MQA)
+
+
+def _double_group(rank, world, intra, dq_groups):
+    """Hierarchical ring: nodes of `intra` consecutive ranks (reference test/test_burst.py:120-156)."""
+    from burst_attn.burst_attn_interface import _Topology, get_partition_id
+    from oracle import attention_oracle as orc
+    os.environ["BA_DOUBLE_RING"] = "1"
+    rows = [list(range(n * intra, (n + 1) * intra)) for n in range(world // intra)]
+    cols = [list(c) for c in zip(*rows)]
+    mk = lambda ranks: dist.new_subgroups_by_enumeration(ranks, backend="gloo")[0]  # noqa: E731
+    double_group = [mk(rows), mk(cols)]
+    if dq_groups:
+        double_group = [(double_group[0], mk(rows)), (double_group[1], mk(cols))]
+    topo = _Topology(None, double_group)
+    assert topo.hier and (topo.L, topo.M) == (intra, world // intra)
+    plain = [g[0] if isinstance(g, tuple) else g for g in double_group]
+    seen = sorted(get_partition_id(plain, r) for r in range(1, world + 1))
+    assert seen == list(range(world)), seen  # every shard is visited exactly once
+    assert get_partition_id(plain, 1) == rank
+    for r in range(1, world + 1):  # the oracle's restatement is pinned to the reference (tests/golden)
+        assert get_partition_id(plain, r) == orc.get_partition_id_double(r, rank % intra, rank // intra, intra,
+                                                                        world // intra)
+    return double_group
+
+
+def _check(ops, rank, world, case, seq_dim, hq, hkv, double_group=(None, None)):
+    """One call of the ring driver on this rank, forward and backward, against dense attention."""
+    from burst_attn import burst_attn_func, burst_attn_func_striped, comm
+    from oracle import attention_oracle as orc
+
+    func, causal, layout = {
+        "none": (burst_attn_func, False, "contiguous"),
+        "zigzag": (burst_attn_func, True, "zigzag"),
+        "striped": (burst_attn_func_striped, True, "striped"),
+    }[case]
+    G = hq // hkv
+    torch.manual_seed(1234)  # same full tensors on every rank (the reference broadcasts from rank 0)
+    B, S, D = 2, 8 * 2 * world, 16
+    q = torch.randn(B, S, hq, D, dtype=torch.float64)
+    k, v = (torch.randn(B, S, hkv, D, dtype=torch.float64) for _ in range(2))
+    do = torch.randn(B, S, hq, D, dtype=torch.float64)
+    scale = D ** -0.5
+    qr, kr, vr = (t.clone().requires_grad_() for t in (q, k, v))
+    o_ref, _ = orc.dense_attention(qr, kr.repeat_interleave(G, dim=2), vr.repeat_interleave(G, dim=2), scale, causal)
+    g_ref = torch.autograd.grad(o_ref, (qr, kr, vr), do)
+
+    def sh(t):
+        x = orc.shard(t, rank, world, layout)
+        return x if seq_dim == 1 else x.permute(0, 2, 1, 3).contiguous()
+
+    def unlay(t):
+        return t if seq_dim == 1 else t.permute(0, 2, 1, 3)
+
+    ql, kl, vl = (sh(t).requires_grad_() for t in (q, k, v))
+    flash = "cuda" if seq_dim == 1 else None
+    posted = []  # bytes handed to the ring per forward hop
+    plain_post = comm.Ring.post
+
+    def post(self, srcs, dsts):
+        posted.append(sum(s.numel() * s.element_size() for s in srcs))
+        return plain_post(self, srcs, dsts)
+
+    ops.calls.clear()
+    comm.Ring.post = post
+    try:
+        o = func(ql, kl, vl, None, flash, causal, True, False, None, list(double_group))
+    finally:
+        comm.Ring.post = plain_post
+    g = torch.autograd.grad(o, (ql, kl, vl), sh(do))
+    tol = dict(rtol=1e-5, atol=1e-5)  # fp32 carried state / accumulators in the driver
+    torch.testing.assert_close(unlay(o.detach()), orc.shard(o_ref.detach(), rank, world, layout), **tol)
+    for got, ref, inp in zip(g, g_ref, (ql, kl, vl)):
+        assert got.shape == inp.shape
+        torch.testing.assert_close(unlay(got), orc.shard(ref, rank, world, layout), **tol)
+    # user inputs must not have been clobbered (the reference reuses k, v, q, dO as receive buffers)
+    torch.testing.assert_close(unlay(kl.detach()), orc.shard(k, rank, world, layout))
+    # forward hops: K and V of this rank's shard, Hkv heads -- 1/G of the MHA hop with the same Hq
+    assert len(posted) == world - 1, posted
+    mha_hop = 2 * B * (S // world) * hq * D * q.element_size()
+    for n in posted:
+        assert n * G == mha_hop, (n, G, mha_hop)
+    # one chunk launch per round, no copies: W forward rounds (+1 cast in the zigzag tail case)
+    nf = sum(1 for c in ops.calls if c[0] == "fwd")
+    nb = sum(1 for c in ops.calls if c[0] == "bwd")
+    if not os.environ.get("BA_TEST_NO_LAUNCH_COUNT"):
+        assert nf == world and nb == world, (nf, nb)
+
+
+def _worker(rank, world, port, errq, case, seq_dim, intra, dq_groups, gqa):
     try:
         for p in (ROOT, os.path.join(ROOT, "burst-attention_b200"), os.path.join(ROOT, "tests")):
             if p not in sys.path:
@@ -74,70 +167,16 @@ def _worker(rank, world, port, case, seq_dim, errq, intra=0, dq_groups=False):
         os.environ["MASTER_ADDR"] = "127.0.0.1"
         os.environ["MASTER_PORT"] = str(port)
         dist.init_process_group("gloo", rank=rank, world_size=world)
-        from burst_attn import burst_attn_func, burst_attn_func_striped, chunk_ops
-        from oracle import attention_oracle as orc
+        from burst_attn import chunk_ops
         from oracle_ops import OracleOps
         ops = OracleOps()
         chunk_ops._set_ops_for_testing(ops)
         if os.environ.get("BA_TEST_DEFERRED"):
             _install_deferred_transport()
-
-        func, causal, layout = {
-            "none": (burst_attn_func, False, "contiguous"),
-            "zigzag": (burst_attn_func, True, "zigzag"),
-            "striped": (burst_attn_func_striped, True, "striped"),
-        }[case]
-        torch.manual_seed(1234)  # same full tensors on every rank (the reference broadcasts from rank 0)
-        B, S, H, D = 2, 8 * 2 * world, 3, 16
-        q, k, v, do = (torch.randn(B, S, H, D, dtype=torch.float64) for _ in range(4))
-        scale = D ** -0.5
-        qr, kr, vr = (t.clone().requires_grad_() for t in (q, k, v))
-        o_ref, _ = orc.dense_attention(qr, kr, vr, scale, causal)
-        g_ref = torch.autograd.grad(o_ref, (qr, kr, vr), do)
-
-        def sh(t):
-            x = orc.shard(t, rank, world, layout)
-            return x if seq_dim == 1 else x.permute(0, 2, 1, 3).contiguous()
-
-        def unlay(t):
-            return t if seq_dim == 1 else t.permute(0, 2, 1, 3)
-
-        ql, kl, vl = (sh(t).requires_grad_() for t in (q, k, v))
-        flash = "cuda" if seq_dim == 1 else None
-        if causal and seq_dim == 2:
-            return  # reference asserts causal needs flash == "cuda"
-        double_group = [None, None]
-        if intra:  # hierarchical ring: nodes of `intra` consecutive ranks (reference test/test_burst.py:120-156)
-            os.environ["BA_DOUBLE_RING"] = "1"  # opt-in (flat ring over process_group is the default)
-            rows = [list(range(n * intra, (n + 1) * intra)) for n in range(world // intra)]
-            cols = [list(c) for c in zip(*rows)]
-            mk = lambda ranks: dist.new_subgroups_by_enumeration(ranks, backend="gloo")[0]  # noqa: E731
-            double_group = [mk(rows), mk(cols)]
-            if dq_groups:
-                double_group = [(double_group[0], mk(rows)), (double_group[1], mk(cols))]
-            from burst_attn.burst_attn_interface import _Topology, get_partition_id
-            topo = _Topology(None, double_group)
-            assert topo.hier and (topo.L, topo.M) == (intra, world // intra)
-            plain = [g[0] if isinstance(g, tuple) else g for g in double_group]
-            seen = sorted(get_partition_id(plain, r) for r in range(1, world + 1))
-            assert seen == list(range(world)), seen  # every shard is visited exactly once
-            assert get_partition_id(plain, 1) == rank
-            for r in range(1, world + 1):  # the oracle's restatement is pinned to the reference (tests/golden)
-                assert get_partition_id(plain, r) == orc.get_partition_id_double(r, rank % intra, rank // intra, intra,
-                                                                                world // intra)
-        o = func(ql, kl, vl, None, flash, causal, True, False, None, double_group)
-        g = torch.autograd.grad(o, (ql, kl, vl), sh(do))
-        tol = dict(rtol=1e-5, atol=1e-5)  # fp32 carried state / accumulators in the driver
-        torch.testing.assert_close(unlay(o.detach()), orc.shard(o_ref.detach(), rank, world, layout), **tol)
-        for got, ref in zip(g, g_ref):
-            torch.testing.assert_close(unlay(got), orc.shard(ref, rank, world, layout), **tol)
-        # user inputs must not have been clobbered (the reference reuses k, v, q, dO as receive buffers)
-        torch.testing.assert_close(unlay(kl.detach()), orc.shard(k, rank, world, layout))
-        # one chunk launch per round, no copies: W forward rounds (+1 cast in the zigzag tail case)
-        nf = sum(1 for c in ops.calls if c[0] == "fwd")
-        nb = sum(1 for c in ops.calls if c[0] == "bwd")
-        if not os.environ.get("BA_TEST_NO_LAUNCH_COUNT"):
-            assert nf == world and nb == world, (nf, nb)
+        double_group = _double_group(rank, world, intra, dq_groups) if intra else (None, None)
+        if not (case != "none" and seq_dim == 2):  # reference asserts causal needs flash == "cuda"
+            for hq, hkv in ([(HQ, h) for h in HKV_CASES] if gqa else [(3, 3)]):
+                _check(ops, rank, world, case, seq_dim, hq, hkv, double_group)
         dist.barrier()
         dist.destroy_process_group()
     except Exception as e:  # noqa: BLE001
@@ -146,22 +185,28 @@ def _worker(rank, world, port, case, seq_dim, errq, intra=0, dq_groups=False):
         raise
 
 
-@pytest.mark.parametrize("world", [2, 4])
-@pytest.mark.parametrize("case", ["none", "zigzag", "striped"])
-def test_ring_driver_matches_dense(world, case):
+def _spawn(world, case, seq_dim=1, intra=0, dq_groups=False, gqa=False):
+    """Run _worker on `world` gloo ranks and fail with every rank's traceback."""
     ctx = mp.get_context("spawn")
     errq = ctx.SimpleQueue()
     port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, case, 1, errq)) for r in range(world)]
+    procs = [ctx.Process(target=_worker, args=(r, world, port, errq, case, seq_dim, intra, dq_groups, gqa))
+             for r in range(world)]
     for p in procs:
         p.start()
     for p in procs:
-        p.join(180)
+        p.join(240)
     errs = []
     while not errq.empty():
         errs.append(errq.get())
     assert not errs, "\n".join(errs)
     assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+
+
+@pytest.mark.parametrize("world", [2, 4])
+@pytest.mark.parametrize("case", ["none", "zigzag", "striped"])
+def test_ring_driver_matches_dense(world, case):
+    _spawn(world, case)
 
 
 @pytest.mark.parametrize("world,intra,case,dq_groups", [
@@ -173,19 +218,7 @@ def test_double_ring_matches_dense(world, intra, case, dq_groups):
     """Hierarchical (double) ring, W = L*M with (L, M) in {(2,2), (3,2), (2,3), (4,2), (2,4)}: K/V and Q-bundle prefetch
     across nodes, dQ node sums chained along the inter-node ring (reference test_burst.py:239-247
     ``double_ring`` axis)."""
-    ctx = mp.get_context("spawn")
-    errq = ctx.SimpleQueue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, case, 1, errq, intra, dq_groups)) for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(240)
-    errs = []
-    while not errq.empty():
-        errs.append(errq.get())
-    assert not errs, "\n".join(errs)
-    assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+    _spawn(world, case, intra=intra, dq_groups=dq_groups)
 
 
 @pytest.mark.parametrize("world,intra,case", [(4, 0, "none"), (4, 0, "zigzag"), (4, 0, "striped"),
@@ -195,35 +228,11 @@ def test_no_buffer_hazards_with_asynchronous_transport(world, intra, case, monke
     destinations at ``post`` (see _install_deferred_transport): what the side-stream transport does on GPUs."""
     monkeypatch.setenv("BA_TEST_DEFERRED", "1")
     monkeypatch.setenv("BA_RING_TRANSPORT", "ce")  # CPU tensors still travel over gloo; turns on the arena check
-    ctx = mp.get_context("spawn")
-    errq = ctx.SimpleQueue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, case, 1, errq, intra, False)) for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(240)
-    errs = []
-    while not errq.empty():
-        errs.append(errq.get())
-    assert not errs, "\n".join(errs)
-    assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+    _spawn(world, case, intra=intra)
 
 
 def test_ring_driver_normal_layout_world2():
-    ctx = mp.get_context("spawn")
-    errq = ctx.SimpleQueue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, "none", 2, errq)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(180)
-    errs = []
-    while not errq.empty():
-        errs.append(errq.get())
-    assert not errs, "\n".join(errs)
-    assert all(p.exitcode == 0 for p in procs)
+    _spawn(2, "none", seq_dim=2)
 
 
 def test_single_process_world1_cpu():
@@ -357,19 +366,7 @@ def test_ring_driver_with_l2_blocking_world2(case, monkeypatch):
     zigzag rounds and the causal offsets compose."""
     monkeypatch.setenv("BA_L2_BLOCK", "8")
     monkeypatch.setenv("BA_TEST_NO_LAUNCH_COUNT", "1")
-    ctx = mp.get_context("spawn")
-    errq = ctx.SimpleQueue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, case, 1, errq)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(180)
-    errs = []
-    while not errq.empty():
-        errs.append(errq.get())
-    assert not errs, "\n".join(errs)
-    assert all(p.exitcode == 0 for p in procs)
+    _spawn(2, case)
 
 
 @pytest.mark.parametrize("blk", [16, 1000])
@@ -419,5 +416,101 @@ def test_single_gpu_wrappers_packed_bias_blocked_cpu(monkeypatch, blk):
             torch.testing.assert_close(a, r, rtol=1e-5, atol=1e-5)
         with pytest.raises(NotImplementedError):
             flash_attn_func(qq, kk, vv, torch.zeros(1, H, 40, S), False)
+    finally:
+        chunk_ops._set_ops_for_testing(None)
+
+
+@pytest.mark.parametrize("case,seq_dim", [("none", 1), ("zigzag", 1), ("striped", 1), ("none", 2)])
+def test_gqa_world1(case, seq_dim):
+    """Grouped-query K/V (Hkv < Hq) through the driver at W = 1, in-process."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from burst_attn import chunk_ops
+    from oracle_ops import OracleOps
+    ops = OracleOps()
+    chunk_ops._set_ops_for_testing(ops)
+    try:
+        for hkv in HKV_CASES:
+            _check(ops, 0, 1, case, seq_dim, HQ, hkv)
+    finally:
+        chunk_ops._set_ops_for_testing(None)
+
+
+@pytest.mark.parametrize("world", [2, 4])
+@pytest.mark.parametrize("case,seq_dim", [("none", 1), ("zigzag", 1), ("striped", 1), ("none", 2)])
+def test_gqa_ring_matches_dense(world, case, seq_dim):
+    _spawn(world, case, seq_dim, gqa=True)
+
+
+@pytest.mark.parametrize("case", ["none", "zigzag", "striped"])
+def test_gqa_double_ring_matches_dense(case):
+    """Hierarchical ring, W = 4 as 2 nodes of 2: K/V (Hkv heads) hop inside the node and prefetch across nodes."""
+    _spawn(4, case, intra=2, gqa=True)
+
+
+@pytest.mark.parametrize("seq_dim", [1, 2])
+def test_q_heads_not_a_multiple_of_kv_heads_raises(seq_dim):
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from burst_attn import burst_attn_func, chunk_ops
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
+    try:
+        q = torch.randn(1, 16, 3, 16, dtype=torch.float64)
+        kv = torch.randn(1, 16, 2, 16, dtype=torch.float64)
+        if seq_dim == 2:
+            q, kv = q.transpose(1, 2).contiguous(), kv.transpose(1, 2).contiguous()
+        with pytest.raises(AssertionError, match="multiple"):
+            burst_attn_func(q, kv, kv, None, "cuda" if seq_dim == 1 else None, False)
+    finally:
+        chunk_ops._set_ops_for_testing(None)
+
+
+@pytest.mark.parametrize("blk", [16, 1000])
+def test_gqa_single_gpu_wrappers_cpu(monkeypatch, blk):
+    """flash_attn_func / flash_attn_kvpacked_func with nheads_k | nheads (flash-attn's GQA), per-key bias per query
+    head, L2 blocking on and off: the Python logic on CPU with the oracle operators; gradients come back with the
+    shapes of the inputs."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from burst_attn import chunk_ops
+    from burst_attn.flash_triton import flash_attn_func, flash_attn_kvpacked_func
+    from oracle import attention_oracle as orc
+    from oracle_ops import OracleOps
+    monkeypatch.setenv("BA_L2_BLOCK", str(blk))
+    ops = OracleOps()
+    ops.tile_head_dims = (16,)
+    chunk_ops._set_ops_for_testing(ops)
+    try:
+        torch.manual_seed(17)
+        B, S, D = 2, 70, 16
+        for hkv in HKV_CASES:
+            G = HQ // hkv
+            q, do = (torch.randn(B, S, HQ, D, dtype=torch.float64) for _ in range(2))
+            kv = torch.randn(B, S, 2, hkv, D, dtype=torch.float64)
+            k, v = kv[:, :, 0].contiguous(), kv[:, :, 1].contiguous()
+            bias = torch.randn(1, HQ, 1, S, dtype=torch.float64)
+            bias[..., 2::7] = float("-inf")
+            for causal in (False, True):
+                qr, kr, vr = (t.clone().requires_grad_() for t in (q, k, v))
+                o_ref, _ = orc.dense_attention(qr, kr.repeat_interleave(G, 2), vr.repeat_interleave(G, 2), None,
+                                               causal, bias=bias)
+                dq, dk, dv = torch.autograd.grad(o_ref, (qr, kr, vr), do)
+                qq, kk, vv = (t.clone().requires_grad_() for t in (q, k, v))
+                o = flash_attn_func(qq, kk, vv, bias, causal)
+                g = torch.autograd.grad(o, (qq, kk, vv), do)
+                torch.testing.assert_close(o.detach(), o_ref.detach(), rtol=1e-5, atol=1e-5)
+                for a, r, inp in zip(g, (dq, dk, dv), (qq, kk, vv)):
+                    assert a.shape == inp.shape
+                    torch.testing.assert_close(a, r, rtol=1e-5, atol=1e-5)
+                qq, pkv = q.clone().requires_grad_(), kv.clone().requires_grad_()
+                o = flash_attn_kvpacked_func(qq, pkv, bias, causal)
+                gq, gkv = torch.autograd.grad(o, (qq, pkv), do)
+                assert gkv.shape == pkv.shape
+                torch.testing.assert_close(gq, dq, rtol=1e-5, atol=1e-5)
+                torch.testing.assert_close(gkv[:, :, 0], dk, rtol=1e-5, atol=1e-5)
+                torch.testing.assert_close(gkv[:, :, 1], dv, rtol=1e-5, atol=1e-5)
+        k2 = torch.randn(B, S, 2, D, dtype=torch.float64)
+        with pytest.raises(AssertionError, match="multiple"):
+            flash_attn_func(q[:, :, :3], k2, k2, None, False)
+        with pytest.raises(AssertionError, match="multiple"):
+            flash_attn_kvpacked_func(q[:, :, :3], torch.stack([k2, k2], dim=2), None, False)
     finally:
         chunk_ops._set_ops_for_testing(None)
