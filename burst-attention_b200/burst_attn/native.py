@@ -38,20 +38,53 @@ class ba_rowstat(ctypes.Structure):
 
 _lib = None
 
-_EXPORTS = (
-    "ba_last_error", "ba_device_check", "ba_version", "ba_fwd_chunk", "ba_fwd_chunk_bias", "ba_bwd_delta", "ba_bwd_chunk",
-    "ba_bwd_chunk_bias", "ba_fwd_chunk_gqa", "ba_bwd_chunk_gqa",
-    "ba_cast_from_f32", "ba_accumulate_f32", "ba_ring_unique_id", "ba_ring_create", "ba_ring_post",
-    "ba_ring_wait", "ba_ring_rank", "ba_ring_world", "ba_ring_destroy", "ba_ring_arena_create",
-    "ba_ring_arena_connect",
-)
+_i, _f, _vp, _i64 = ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_int64
+_T4, _RS, _PVP = ba_tensor4, ba_rowstat, ctypes.POINTER(ctypes.c_void_p)
+# name -> (restype, argtypes) of every function include/burst_attn_b200.h declares, in its order
+# (tests/test_native_abi.py checks each signature against the header)
+_EXPORTS = {
+    "ba_last_error": (ctypes.c_char_p, []),
+    "ba_device_check": (_i, []),
+    "ba_version": (_i, []),
+    "ba_fwd_chunk": (_i, [_T4, _T4, _T4, _T4, _RS, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_fwd_chunk_bias": (_i, [_T4, _T4, _T4, _RS, _T4, _RS, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_fwd_chunk_gqa": (_i, [_T4, _T4, _T4, _RS, _T4, _RS, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_bwd_delta": (_i, [_T4, _T4, _RS, _i, _i, _i, _i, _i, _vp]),
+    "ba_bwd_chunk": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _T4, _T4, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_bwd_chunk_bias": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _RS, _T4, _T4, _T4,
+                               _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_bwd_chunk_gqa": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _RS, _T4, _T4, _T4,
+                              _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_cast_from_f32": (_i, [_T4, _T4, _i, _i, _i, _i, _i, _vp]),
+    "ba_accumulate_f32": (_i, [_T4, _T4, _i, _i, _i, _i, _vp]),
+    "ba_ring_unique_id": (_i, [_vp]),
+    "ba_ring_create": (_i, [_vp, _i, _i, _PVP]),
+    "ba_ring_post": (_i, [_vp, _PVP, _PVP, ctypes.POINTER(_i64), _i, _vp]),
+    "ba_ring_wait": (_i, [_vp, _vp]),
+    "ba_ring_rank": (_i, [_vp]),
+    "ba_ring_world": (_i, [_vp]),
+    "ba_ring_destroy": (_i, [_vp]),
+    "ba_ring_arena_create": (_i, [_vp, _i64, _PVP, _vp]),
+    "ba_ring_arena_connect": (_i, [_vp, _vp, _vp]),
+}
 SELFTEST_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libburst_attn_b200_selftest.so")
-_SELFTEST_EXPORTS = ("ba_selftest_last_error", "ba_selftest")
+# the same for include/burst_attn_b200_selftest.h
+_SELFTEST_EXPORTS = {
+    "ba_selftest_last_error": (ctypes.c_char_p, []),
+    "ba_selftest": (_i, [_i, _vp, _vp, _vp, _i, _vp]),
+}
+
+
+def _bind(L: ctypes.CDLL, signatures) -> ctypes.CDLL:
+    for name, (restype, argtypes) in signatures.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return L
 
 
 def exported_symbols() -> Sequence[str]:
     """Every symbol include/burst_attn_b200.h declares (checked by the CPU tests)."""
-    return _EXPORTS
+    return tuple(_EXPORTS)
 
 
 def lib() -> ctypes.CDLL:
@@ -62,56 +95,8 @@ def lib() -> ctypes.CDLL:
         raise NativeLibraryError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(or `make -C burst-attention_b200/csrc`).  There is no CPU/PyTorch fallback.")
-    L = ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_GLOBAL)
-    i, f, vp = ctypes.c_int, ctypes.c_float, ctypes.c_void_p
-    L.ba_last_error.restype = ctypes.c_char_p
-    L.ba_last_error.argtypes = []
-    L.ba_device_check.restype = i
-    L.ba_version.restype = i
-    L.ba_fwd_chunk.restype = i
-    L.ba_fwd_chunk.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_tensor4,
-                               i, i, i, i, i, f, i, i, i, i, vp]
-    L.ba_fwd_chunk_bias.restype = i
-    L.ba_fwd_chunk_bias.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_tensor4, ba_rowstat, ba_tensor4,
-                                    i, i, i, i, i, f, i, i, i, i, vp]
-    L.ba_bwd_chunk_bias.restype = i
-    L.ba_bwd_chunk_bias.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_rowstat, ba_rowstat,
-                                    ba_tensor4, ba_tensor4, ba_tensor4, i, i, i, i, i, f, i, i, i, i, vp]
-    L.ba_fwd_chunk_gqa.restype = i
-    L.ba_fwd_chunk_gqa.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_tensor4, ba_rowstat, ba_tensor4,
-                                   i, i, i, i, i, i, f, i, i, i, i, vp]
-    L.ba_bwd_chunk_gqa.restype = i
-    L.ba_bwd_chunk_gqa.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_rowstat, ba_rowstat,
-                                   ba_tensor4, ba_tensor4, ba_tensor4, i, i, i, i, i, i, f, i, i, i, i, vp]
-    L.ba_bwd_delta.restype = i
-    L.ba_bwd_delta.argtypes = [ba_tensor4, ba_tensor4, ba_rowstat, i, i, i, i, i, vp]
-    L.ba_bwd_chunk.restype = i
-    L.ba_bwd_chunk.argtypes = [ba_tensor4, ba_tensor4, ba_tensor4, ba_tensor4, ba_rowstat, ba_rowstat,
-                               ba_tensor4, ba_tensor4, ba_tensor4, i, i, i, i, i, f, i, i, i, i, vp]
-    L.ba_cast_from_f32.restype = i
-    L.ba_cast_from_f32.argtypes = [ba_tensor4, ba_tensor4, i, i, i, i, i, vp]
-    L.ba_accumulate_f32.restype = i
-    L.ba_accumulate_f32.argtypes = [ba_tensor4, ba_tensor4, i, i, i, i, vp]
-    L.ba_ring_unique_id.restype = i
-    L.ba_ring_unique_id.argtypes = [vp]
-    L.ba_ring_create.restype = i
-    L.ba_ring_create.argtypes = [vp, i, i, ctypes.POINTER(vp)]
-    L.ba_ring_post.restype = i
-    L.ba_ring_post.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int64), i, vp]
-    L.ba_ring_wait.restype = i
-    L.ba_ring_wait.argtypes = [vp, vp]
-    L.ba_ring_rank.restype = i
-    L.ba_ring_rank.argtypes = [vp]
-    L.ba_ring_world.restype = i
-    L.ba_ring_world.argtypes = [vp]
-    L.ba_ring_destroy.restype = i
-    L.ba_ring_destroy.argtypes = [vp]
-    L.ba_ring_arena_create.restype = i
-    L.ba_ring_arena_create.argtypes = [vp, ctypes.c_int64, ctypes.POINTER(vp), vp]
-    L.ba_ring_arena_connect.restype = i
-    L.ba_ring_arena_connect.argtypes = [vp, vp, vp]
-    _lib = L
-    return L
+    _lib = _bind(ctypes.CDLL(LIB_PATH, mode=ctypes.RTLD_GLOBAL), _EXPORTS)
+    return _lib
 
 
 _selftest_lib = None
@@ -123,12 +108,7 @@ def selftest_lib() -> ctypes.CDLL:
     if _selftest_lib is None:
         if not os.path.exists(SELFTEST_LIB_PATH):
             raise NativeLibraryError(f"{SELFTEST_LIB_PATH} not found: build with __graft_entry__.build()")
-        L = ctypes.CDLL(SELFTEST_LIB_PATH)
-        i, vp = ctypes.c_int, ctypes.c_void_p
-        L.ba_selftest_last_error.restype = ctypes.c_char_p
-        L.ba_selftest.restype = i
-        L.ba_selftest.argtypes = [i, vp, vp, vp, i, vp]
-        _selftest_lib = L
+        _selftest_lib = _bind(ctypes.CDLL(SELFTEST_LIB_PATH), _SELFTEST_EXPORTS)
     return _selftest_lib
 
 

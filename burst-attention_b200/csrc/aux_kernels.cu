@@ -96,12 +96,6 @@ accumulate_kernel(const float* __restrict__ src, int64_t s_sb, int64_t s_ss, int
   *pd = y;
 }
 
-static bool aligned16(const ba_tensor4& t, int esize) {
-  const int q = 16 / esize;
-  return (reinterpret_cast<uintptr_t>(t.ptr) & 15) == 0 && t.stride_b % q == 0 && t.stride_s % q == 0 &&
-         t.stride_h % q == 0;
-}
-
 }  // namespace ba
 
 extern "C" int ba_bwd_delta(ba_tensor4 o, ba_tensor4 d_o, ba_rowstat delta, int B, int S, int H, int D, int dtype,

@@ -42,16 +42,6 @@ namespace ba {
 constexpr int kBwdThreads = 384;  // warpgroup 0: loader (warp 0); warpgroups 1, 2: MMA + element-wise
 constexpr int kBwdN = 128;        // keys per CTA
 constexpr int kBwdM = 64;         // query rows per block of the Q-bundle
-constexpr float kBwdLog2e = 1.4426950408889634f;
-
-template <int N>
-__device__ __forceinline__ void reg_inc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
-}
-template <int N>
-__device__ __forceinline__ void reg_dec() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
-}
 
 struct BwdParams {
   const float* lse;
@@ -160,7 +150,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 
   if (warp < 4) {
     // ============================================================ loader (warp 0)
-    reg_dec<24>();
+    reg_alloc_dec<24>();
     if (warp != 0) return;
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->kv_full, 2 * kBoxes * kBoxKV);
@@ -185,7 +175,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
           dl = __ldg(p.delta + (int64_t)b * p.dl_sb + (int64_t)h * p.dl_sh + row);
           if (l == -INFINITY) l = INFINITY;
         }
-        stat[lane + 32 * j] = l * kBwdLog2e;
+        stat[lane + 32 * j] = l * kLog2e;
         stat[kBwdM + lane + 32 * j] = dl;
       }
       __syncwarp();
@@ -203,7 +193,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   }
 
   // ============================================================ consumers (64 keys per warpgroup)
-  reg_inc<240>();
+  reg_alloc_inc<240>();
   const int wg = (threadIdx.x >> 7) - 1;
   const int tid = threadIdx.x & 127;
   const int w = warp & 3, g = lane >> 2, t = lane & 3;
@@ -235,7 +225,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 #pragma unroll
       for (int r = 0; r < 2; ++r)
         bias2[r] = (p.bias && keys[r] < p.Sk)
-                       ? __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + keys[r]) * kBwdLog2e
+                       ? __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + keys[r]) * kLog2e
                        : 0.f;
     }
     mbar_wait(&bars->q_full[st], (step >> 1) & 1);
@@ -419,23 +409,18 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   }
 }
 
-template <bool kBF16, int kD>
-static int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+static int launch_bwd(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                       const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream) {
-  auto kern = bwd_chunk_kernel<kBF16, kD>;
-  constexpr int smem = BwdLayout<kD>::kSmemBytes;
+  const bool bf16 = dtype == BA_DTYPE_BF16;
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, BwdParams) =
+      D == 64 ? (bf16 ? bwd_chunk_kernel<true, 64> : bwd_chunk_kernel<false, 64>)
+              : (bf16 ? bwd_chunk_kernel<true, 128> : bwd_chunk_kernel<false, 128>);
+  const int smem = D == 64 ? BwdLayout<64>::kSmemBytes : BwdLayout<128>::kSmemBytes;
   BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   dim3 grid((p.Sk + kBwdN - 1) / kBwdN, p.H / p.G, p.B);  // one CTA per (key block, K/V head, batch)
   kern<<<grid, kBwdThreads, smem, stream>>>(tmQ, tmK, tmV, tmDO, tmDQ, p);
   BA_CHECK_CUDA(cudaGetLastError());
   return BA_OK;
-}
-
-template <int kD>
-static int launch_bwd_dt(int dtype, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                         const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream) {
-  return dtype == BA_DTYPE_BF16 ? launch_bwd<true, kD>(tmQ, tmK, tmV, tmDO, tmDQ, p, stream)
-                                : launch_bwd<false, kD>(tmQ, tmK, tmV, tmDO, tmDQ, p, stream);
 }
 
 // Deterministic-mode workspace (turn counters + tickets), one per (device, stream), grown on demand, zeroed on
@@ -472,11 +457,6 @@ static int* bwd_sem_workspace(size_t n_ints, cudaStream_t stream) {
   return w->ptr;
 }
 
-static bool f32_view_ok(const ba_tensor4& t) {
-  return t.ptr && (reinterpret_cast<uintptr_t>(t.ptr) & 15) == 0 && t.stride_b % 4 == 0 && t.stride_s % 4 == 0 &&
-         t.stride_h % 4 == 0;
-}
-
 }  // namespace ba
 
 extern "C" int ba_bwd_chunk(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
@@ -501,20 +481,15 @@ extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_t
                                 ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
                                 int mask_mode, int causal_offset, int flags, int dtype, void* stream) {
   using namespace ba;
-  BA_REQUIRE(H_kv > 0 && H % H_kv == 0, "ba_bwd_chunk: H_kv=%d must be positive and divide H=%d", H_kv, H);
-  BA_REQUIRE(D == 128 || D == 64, "ba_bwd_chunk: head dim %d unsupported (64 or 128)", D);
-  BA_REQUIRE(B > 0 && Sq > 0 && Sk > 0 && H > 0, "ba_bwd_chunk: empty problem B=%d Sq=%d Sk=%d H=%d", B, Sq, Sk, H);
-  BA_REQUIRE(dtype == BA_DTYPE_FP16 || dtype == BA_DTYPE_BF16, "ba_bwd_chunk: bad dtype %d", dtype);
-  BA_REQUIRE(mask_mode == BA_MASK_NONE || mask_mode == BA_MASK_CAUSAL, "ba_bwd_chunk: bad mask mode %d", mask_mode);
-  BA_REQUIRE(scale > 0.f && isfinite(scale), "ba_bwd_chunk: softmax scale must be positive and finite");
+  int rc;
+  if ((rc = check_chunk_args("ba_bwd_chunk", B, Sq, Sk, H, H_kv, D, scale, mask_mode, dtype))) return rc;
   BA_REQUIRE(d_o.ptr && q.ptr && k.ptr && v.ptr && delta.ptr && lse.ptr, "ba_bwd_chunk: null input");
-  BA_REQUIRE(f32_view_ok(dq_acc) && f32_view_ok(dk_acc) && f32_view_ok(dv_acc),
+  BA_REQUIRE(dq_acc.ptr && dk_acc.ptr && dv_acc.ptr && aligned16(dq_acc, 4) && aligned16(dk_acc, 4) &&
+                 aligned16(dv_acc, 4),
              "ba_bwd_chunk: fp32 accumulators must be non-null, 16-byte aligned, strides multiple of 4");
-  BA_REQUIRE(H <= 65535 && B <= 65535, "ba_bwd_chunk: H and B must be <= 65535");
 
   CUtensorMap tmQ, tmK, tmV, tmDO, tmDQ;
   const CUtensorMapDataType dt = lowp_dtype(dtype);
-  int rc;
   if ((rc = make_tensor_map(&tmQ, q, B, Sq, H, D, dt, 2, 64, kBwdM, true))) return rc;
   if ((rc = make_tensor_map(&tmDO, d_o, B, Sq, H, D, dt, 2, 64, kBwdM, true))) return rc;
   if ((rc = make_tensor_map(&tmK, k, B, Sk, H_kv, D, dt, 2, 64, kBwdN, true))) return rc;
@@ -534,7 +509,7 @@ extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_t
   p.B = B, p.Sq = Sq, p.Sk = Sk, p.H = H;
   p.G = H / H_kv;
   p.scale = scale;
-  p.scale_log2 = scale * kBwdLog2e;
+  p.scale_log2 = scale * kLog2e;
   p.causal = mask_mode == BA_MASK_CAUSAL;
   p.causal_off = causal_offset;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -549,6 +524,5 @@ extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_t
       return BA_ERR_CUDA;
     }
   }
-  if (D == 64) return launch_bwd_dt<64>(dtype, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
-  return launch_bwd_dt<128>(dtype, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
+  return launch_bwd(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
 }

@@ -22,11 +22,35 @@
 #include <math.h>
 #include <stdlib.h>
 
-#include "fwd_common.cuh"
 #include "host_common.h"
 #include "sm90_ptx.cuh"
 
 namespace ba {
+
+constexpr int kBlockM = 128;  // Q rows per CTA (64 per consumer warpgroup)
+constexpr int kBlockN = 128;  // keys per K/V tile
+constexpr int kKStages = 2;
+constexpr int kVStages = 2;
+constexpr int kBoxBytes = 128 * 64 * 2;  // 16 KiB: one 128 x 64 SW128 TMA box (a [128][head_dim] tile is head_dim/64 boxes)
+constexpr int kFwdThreads = 384;         // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + softmax
+
+struct FwdParams {
+  float* o_acc;
+  int64_t oacc_sb, oacc_ss, oacc_sh;
+  float* lse;
+  int64_t lse_sb, lse_sh;
+  void* o_out;
+  int64_t oout_sb, oout_ss, oout_sh;
+  int B, Sq, Sk, H;
+  int G;              // query heads per K/V head (grouped-query attention; 1 = MHA): head h reads K/V head h / G
+  float scale_log2;
+  const float* bias;  // optional additive bias per key [B|1, H, Sk] (fp32, indexed by the query head), or null
+  int64_t bias_sb, bias_sh;
+  int causal;
+  int causal_off;
+  int load_state;
+  int store_lowp;
+};
 
 struct __align__(8) FwdBarriers {
   uint64_t q_full;
@@ -50,15 +74,6 @@ struct FwdLayout {
   static constexpr int kSmemBytes = kOffBars + 256 /*barriers*/;
   static_assert(kSmemBytes <= 232448, "forward kernel exceeds 227 KiB of shared memory");
 };
-
-template <int N>
-__device__ __forceinline__ void reg_alloc_inc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
-}
-template <int N>
-__device__ __forceinline__ void reg_alloc_dec() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
-}
 
 // number of 128-key tiles the 64 Q rows starting at r0 must visit
 __device__ __forceinline__ int fwd_trip_count(int r0, const FwdParams& p) {
@@ -314,11 +329,17 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 }
 
 
-template <bool kBF16, int kD, bool kBias>
-static int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdParams& p,
-                      cudaStream_t stream) {
-  auto kern = fwd_chunk_kernel<kBF16, kD, kBias>;
-  constexpr int smem = FwdLayout<kD>::kSmemBytes;
+static int launch_fwd(int dtype, int D, bool bias, const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                      const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream) {
+  const bool bf16 = dtype == BA_DTYPE_BF16;
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams);
+  if (bias)
+    kern = D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, true> : fwd_chunk_kernel<false, 64, true>)
+                   : (bf16 ? fwd_chunk_kernel<true, 128, true> : fwd_chunk_kernel<false, 128, true>);
+  else
+    kern = D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, false> : fwd_chunk_kernel<false, 64, false>)
+                   : (bf16 ? fwd_chunk_kernel<true, 128, false> : fwd_chunk_kernel<false, 128, false>);
+  const int smem = D == 64 ? FwdLayout<64>::kSmemBytes : FwdLayout<128>::kSmemBytes;
   BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   dim3 grid((p.Sq + kBlockM - 1) / kBlockM, p.H, p.B);
   kern<<<grid, kFwdThreads, smem, stream>>>(tmQ, tmK, tmV, p);
@@ -327,13 +348,6 @@ static int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUte
 }
 
 }  // namespace ba
-
-template <int kD, bool kBias>
-static int launch_fwd_dt(int dtype, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                         const ba::FwdParams& p, cudaStream_t st) {
-  return dtype == BA_DTYPE_BF16 ? ba::launch_fwd<true, kD, kBias>(tmQ, tmK, tmV, p, st)
-                                : ba::launch_fwd<false, kD, kBias>(tmQ, tmK, tmV, p, st);
-}
 
 extern "C" int ba_fwd_chunk(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse,
                             ba_tensor4 o_out, int B, int Sq, int Sk, int H, int D, float scale, int mask_mode,
@@ -354,29 +368,19 @@ extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_row
                                 ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D,
                                 float scale, int mask_mode, int causal_offset, int flags, int dtype, void* stream) {
   using namespace ba;
-  BA_REQUIRE(H_kv > 0 && H % H_kv == 0, "ba_fwd_chunk: H_kv=%d must be positive and divide H=%d", H_kv, H);
-  BA_REQUIRE(D == 128 || D == 64, "ba_fwd_chunk: head dim %d unsupported (64 or 128)", D);
-  BA_REQUIRE(B > 0 && Sq > 0 && Sk > 0 && H > 0, "ba_fwd_chunk: empty problem B=%d Sq=%d Sk=%d H=%d", B, Sq, Sk, H);
-  BA_REQUIRE(dtype == BA_DTYPE_FP16 || dtype == BA_DTYPE_BF16, "ba_fwd_chunk: bad dtype %d", dtype);
-  BA_REQUIRE(mask_mode == BA_MASK_NONE || mask_mode == BA_MASK_CAUSAL, "ba_fwd_chunk: bad mask mode %d", mask_mode);
-  BA_REQUIRE(scale > 0.f && isfinite(scale), "ba_fwd_chunk: softmax scale must be positive and finite");
+  int rc;
+  if ((rc = check_chunk_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, mask_mode, dtype))) return rc;
   BA_REQUIRE(q.ptr && k.ptr && v.ptr && lse.ptr, "ba_fwd_chunk: null q/k/v/lse");
   const bool first = flags & BA_FWD_FIRST, last = flags & BA_FWD_LAST;
   BA_REQUIRE(!last || o_out.ptr, "ba_fwd_chunk: BA_FWD_LAST needs o_out");
   BA_REQUIRE((first && last) || o_acc.ptr, "ba_fwd_chunk: fp32 state o_acc required unless FIRST|LAST");
-  BA_REQUIRE(H <= 65535 && B <= 65535, "ba_fwd_chunk: H and B must be <= 65535");
   if (o_acc.ptr)
-    BA_REQUIRE((reinterpret_cast<uintptr_t>(o_acc.ptr) & 15) == 0 && o_acc.stride_s % 4 == 0 &&
-                   o_acc.stride_h % 4 == 0 && o_acc.stride_b % 4 == 0,
-               "ba_fwd_chunk: o_acc must be 16-byte aligned with strides multiple of 4 elements");
+    BA_REQUIRE(aligned16(o_acc, 4), "ba_fwd_chunk: o_acc must be 16-byte aligned with strides multiple of 4 elements");
   if (o_out.ptr)
-    BA_REQUIRE((reinterpret_cast<uintptr_t>(o_out.ptr) & 15) == 0 && o_out.stride_s % 8 == 0 &&
-                   o_out.stride_h % 8 == 0 && o_out.stride_b % 8 == 0,
-               "ba_fwd_chunk: o_out must be 16-byte aligned with strides multiple of 8 elements");
+    BA_REQUIRE(aligned16(o_out, 2), "ba_fwd_chunk: o_out must be 16-byte aligned with strides multiple of 8 elements");
 
   CUtensorMap tmQ, tmK, tmV;
   const CUtensorMapDataType dt = lowp_dtype(dtype);
-  int rc;
   if ((rc = make_tensor_map(&tmQ, q, B, Sq, H, D, dt, 2, 64, kBlockM, true))) return rc;
   if ((rc = make_tensor_map(&tmK, k, B, Sk, H_kv, D, dt, 2, 64, kBlockN, true))) return rc;
   if ((rc = make_tensor_map(&tmV, v, B, Sk, H_kv, D, dt, 2, 64, kBlockN, true))) return rc;
@@ -395,9 +399,6 @@ extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_row
   p.causal_off = causal_offset;
   p.load_state = first ? 0 : 1;
   p.store_lowp = last ? 1 : 0;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   p.bias = key_bias.ptr, p.bias_sb = key_bias.stride_b, p.bias_sh = key_bias.stride_h;
-  if (key_bias.ptr)
-    return D == 64 ? launch_fwd_dt<64, true>(dtype, tmQ, tmK, tmV, p, st) : launch_fwd_dt<128, true>(dtype, tmQ, tmK, tmV, p, st);
-  return D == 64 ? launch_fwd_dt<64, false>(dtype, tmQ, tmK, tmV, p, st) : launch_fwd_dt<128, false>(dtype, tmQ, tmK, tmV, p, st);
+  return launch_fwd(dtype, D, key_bias.ptr != nullptr, tmQ, tmK, tmV, p, static_cast<cudaStream_t>(stream));
 }

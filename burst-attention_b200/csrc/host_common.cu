@@ -1,5 +1,6 @@
 #include "host_common.h"
 
+#include <math.h>
 #include <mutex>
 #include <string.h>
 
@@ -72,6 +73,18 @@ int make_tensor_map(CUtensorMap* out, const ba_tensor4& t, int B, int S, int H, 
               box_d, box_s);
     return BA_ERR_CUDA;
   }
+  return BA_OK;
+}
+
+int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
+                     int dtype) {
+  BA_REQUIRE(H_kv > 0 && H % H_kv == 0, "%s: H_kv=%d must be positive and divide H=%d", fn, H_kv, H);
+  BA_REQUIRE(D == 128 || D == 64, "%s: head dim %d unsupported (64 or 128)", fn, D);
+  BA_REQUIRE(B > 0 && Sq > 0 && Sk > 0 && H > 0, "%s: empty problem B=%d Sq=%d Sk=%d H=%d", fn, B, Sq, Sk, H);
+  BA_REQUIRE(dtype == BA_DTYPE_FP16 || dtype == BA_DTYPE_BF16, "%s: bad dtype %d", fn, dtype);
+  BA_REQUIRE(mask_mode == BA_MASK_NONE || mask_mode == BA_MASK_CAUSAL, "%s: bad mask mode %d", fn, mask_mode);
+  BA_REQUIRE(scale > 0.f && isfinite(scale), "%s: softmax scale must be positive and finite", fn);
+  BA_REQUIRE(H <= 65535 && B <= 65535, "%s: H and B must be <= 65535", fn);  // gridDim.y / gridDim.z
   return BA_OK;
 }
 

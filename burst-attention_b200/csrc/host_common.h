@@ -1,6 +1,6 @@
 // Host-side helpers shared by the C-ABI entry points: thread-local error string,
-// CUDA error mapping, and TMA tensor-map construction through the driver entry
-// point (no link-time dependency on libcuda).
+// CUDA error mapping, argument checks, and TMA tensor-map construction through
+// the driver entry point (no link-time dependency on libcuda).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -39,5 +39,18 @@ int make_tensor_map(CUtensorMap* out, const ba_tensor4& t, int B, int S, int H, 
 inline CUtensorMapDataType lowp_dtype(int dtype) {
   return dtype == BA_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
 }
+
+// A view the kernels can access with 16-byte loads and stores: 16-byte aligned base, every stride a multiple of
+// 16 bytes (esize: element size in bytes).  A null pointer passes; callers that need one check for it.
+inline bool aligned16(const ba_tensor4& t, int esize) {
+  const int q = 16 / esize;
+  return (reinterpret_cast<uintptr_t>(t.ptr) & 15) == 0 && t.stride_b % q == 0 && t.stride_s % q == 0 &&
+         t.stride_h % q == 0;
+}
+
+// Preconditions shared by the forward and backward chunk entry points; `fn` names the entry point in the error
+// message.  Returns BA_OK or BA_ERR_INVALID.
+int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
+                     int dtype);
 
 }  // namespace ba

@@ -1,6 +1,7 @@
 """CPU-side checks of the C-ABI boundary: the shared library loads, exports every
-symbol include/burst_attn_b200.h declares, and rejects bad arguments with an
-error string instead of crashing.  No compute call is made (no GPU here)."""
+symbol include/burst_attn_b200.h declares, its ctypes binding has the header's
+signatures, and it rejects bad arguments with an error string instead of
+crashing.  No compute call is made (no GPU here)."""
 import ctypes
 import os
 import re
@@ -9,11 +10,42 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, "include", "burst_attn_b200.h")
+SELFTEST_HEADER = os.path.join(ROOT, "include", "burst_attn_b200_selftest.h")
 
 
 def _declared():
     src = open(HEADER).read()
     return sorted(set(re.findall(r"\b(ba_[a-z0-9_]+)\s*\(", src)))
+
+
+def _prototypes(path):
+    """{name: (return type, [parameter types])} of the functions a C header declares, types with their names
+    dropped and whitespace normalised, e.g. "const void* const*"."""
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", "", open(path).read(), flags=re.S)
+    src = re.sub(r"^\s*#.*$", "", src, flags=re.M)
+    out = {}
+    for ret, name, params in re.findall(r"([A-Za-z_][\w\s*]*?)\s*\b(ba_\w+)\s*\(([^)]*)\)\s*;", src):
+        params = [] if params.strip() == "void" else [p.strip() for p in params.split(",")]
+        types = [" ".join(re.sub(r"\*", " * ", re.sub(r"\s*\w+$", "", p)).split()).replace(" *", "*")
+                 for p in params]
+        out[name] = (" ".join(ret.split()), types)
+    return out
+
+
+def _ctype(nat, c_type, ret=False):
+    """The ctypes type a C type maps to: structs by value, scalars, and pointers as c_void_p except
+    int64_t* (POINTER(c_int64)), pointers to pointers (POINTER(c_void_p)) and a returned string."""
+    base = " ".join(w for w in c_type.replace("*", " ").split() if w != "const")
+    depth = c_type.count("*")
+    if ret and c_type == "const char*":
+        return ctypes.c_char_p
+    if depth == 0:
+        return {"int": ctypes.c_int, "float": ctypes.c_float, "int64_t": ctypes.c_int64,
+                "ba_tensor4": nat.ba_tensor4, "ba_rowstat": nat.ba_rowstat}[base]
+    if depth == 1:
+        return ctypes.POINTER(ctypes.c_int64) if base == "int64_t" else ctypes.c_void_p
+    assert depth == 2, c_type
+    return ctypes.POINTER(ctypes.c_void_p)
 
 
 @pytest.fixture(scope="module")
@@ -48,6 +80,19 @@ def test_selftest_library_is_separate_from_the_product(nat):
         assert not hasattr(L, name), f"{name} must not be exported by the product library"
 
 
+def test_binding_signatures_match_header(nat):
+    """Every bound function's restype and argtypes are the ctypes form of its prototype in the header: ctypes
+    itself checks neither, so a wrong or missing argument type would pass garbage to the library."""
+    for header, L in ((HEADER, nat.lib()), (SELFTEST_HEADER, nat.selftest_lib())):
+        protos = _prototypes(header)
+        assert protos, header
+        for name, (ret, params) in protos.items():
+            fn = getattr(L, name)
+            assert fn.restype is _ctype(nat, ret, ret=True), (name, ret, fn.restype)
+            assert fn.argtypes is not None, f"{name}: argtypes not set"
+            assert list(fn.argtypes) == [_ctype(nat, p) for p in params], (name, params, fn.argtypes)
+
+
 def test_bad_arguments_return_error_string(nat):
     L = nat.lib()
     z4 = nat.ba_tensor4(None, 0, 0, 0)
@@ -63,6 +108,38 @@ def test_bad_arguments_return_error_string(nat):
     rc = L.ba_ring_arena_connect(None, None, None)
     assert rc != 0 and b"ba_ring_arena_connect" in L.ba_last_error()
     assert L.ba_version() >= 200
+
+
+def test_gqa_symbols_exported_and_bound(nat):
+    L = ctypes.CDLL(nat.LIB_PATH)
+    for name in ("ba_fwd_chunk_gqa", "ba_bwd_chunk_gqa"):
+        assert hasattr(L, name), name
+        assert name in nat.exported_symbols()
+    assert nat.lib().ba_version() >= 201
+
+
+@pytest.mark.parametrize("H,H_kv", [(32, 5), (4, 8), (8, 0), (8, -2)])
+def test_bad_kv_head_count_returns_error_string(nat, H, H_kv):
+    """A K/V head count that is not positive or does not divide the query head count is rejected with an error
+    string naming H_kv before anything touches the GPU."""
+    L = nat.lib()
+    z4 = nat.ba_tensor4(None, 0, 0, 0)
+    zr = nat.ba_rowstat(None, 0, 0)
+    rc = L.ba_fwd_chunk_gqa(z4, z4, z4, zr, z4, zr, z4, 1, 128, 128, H, H_kv, 128, 1.0, 0, 0, 3, 1, None)
+    assert rc != 0 and b"H_kv" in L.ba_last_error()
+    rc = L.ba_bwd_chunk_gqa(z4, z4, z4, z4, zr, zr, zr, z4, z4, z4, 1, 128, 128, H, H_kv, 128, 1.0, 0, 0, 0, 1, None)
+    assert rc != 0 and b"H_kv" in L.ba_last_error()
+
+
+def test_valid_kv_head_count_reaches_the_next_check(nat):
+    """H % H_kv == 0 passes the head check: the call then fails on the null operands, not on H_kv."""
+    L = nat.lib()
+    z4 = nat.ba_tensor4(None, 0, 0, 0)
+    zr = nat.ba_rowstat(None, 0, 0)
+    rc = L.ba_fwd_chunk_gqa(z4, z4, z4, zr, z4, zr, z4, 1, 128, 128, 32, 8, 128, 1.0, 0, 0, 3, 1, None)
+    assert rc != 0 and b"null" in L.ba_last_error()
+    rc = L.ba_bwd_chunk_gqa(z4, z4, z4, z4, zr, zr, zr, z4, z4, z4, 1, 128, 128, 32, 1, 128, 1.0, 0, 0, 0, 1, None)
+    assert rc != 0 and b"null" in L.ba_last_error()
 
 
 def test_missing_library_fails_loudly(nat, monkeypatch):
