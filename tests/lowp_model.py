@@ -1,0 +1,589 @@
+"""A 16-bit rounding model of the tile kernels, and the comparator the tile-edge tests use.
+
+``lowp_forward`` / ``lowp_backward`` restate what ``fwd_chunk_kernel`` (csrc/fwd_sm90.cu) and ``bwd_chunk_kernel``
+(csrc/bwd_sm90.cu) compute, rounding at the same points the kernels round and nowhere else:
+
+* scores are fp32 products of the 16-bit inputs, taken to log2 units with the fp32 ``scale * log2(e)``; a key bias
+  is added in log2 units;
+* forward: the softmax runs in fp32; its row sum ``l`` adds the unrounded P; P is rounded to the input dtype
+  (``pack2``) before ``P V``, which accumulates in fp32; the carried state enters as ``m = lse log2(e)``, ``l = 1``,
+  ``acc = o_acc`` (fp32, normalised); O is rounded once, at the end of the last chunk;
+* backward: delta = rowsum(O dO) in fp32 from the 16-bit O; P is recomputed in fp32 from the final lse; ``dV`` uses P
+  rounded to 16 bit; ``dS = P (dP - delta)`` is rounded to 16 bit before both ``dQ = dS K`` and ``dK = dS^T Q``, which
+  accumulate in fp32 and are multiplied by the (fp32) scale.
+
+The model does not reproduce the kernels' order of fp32 operations (the kernel rounds P relative to the running
+maximum of its key tile, the model relative to the final row maximum), so it is a yardstick of the same error
+magnitude, not a bitwise twin.  The truth is ``oracle/attention_oracle.py`` in fp64 on the same 16-bit inputs.
+
+Masks follow the oracle: ``None`` or ``("causal_offset", off)`` (key b visible to row a iff ``b <= a + off``).
+Tensors are in the flash layout ``[B, S, H, D]``; K/V may have fewer heads than Q (query head h reads K/V head
+``h // G``).  Both functions run on whatever device their inputs live on.
+
+``mutant`` injects one realistic kernel fault into the model (``MUTANTS``); ``tests/test_lowp_model.py`` shows that
+the comparator rejects each of them.
+"""
+from __future__ import annotations
+
+import torch
+
+from oracle import attention_oracle as orc
+
+LOG2E = 1.4426950408889634
+LN2 = 0.6931471805599453
+NEG_INF = float("-inf")
+
+# One realistic fault each, for the comparator's own tests.  "_fwd" / "_bwd": only that kernel has the fault.
+MUTANTS = (
+    "drop_key_127",         # key 127 never contributes (forward and backward)
+    "drop_key_128",         # key 128 never contributes
+    "drop_key_last",        # the last key (the ragged tail) never contributes
+    "causal_plus1_fwd",     # forward causal limit one key too large
+    "causal_minus1_fwd",    # forward causal limit one key too small
+    "causal_plus1_bwd",     # backward causal mask lets one key too many through
+    "causal_minus1_bwd",    # backward causal mask drops the diagonal key
+    "strict_swap",          # b < a + off where b <= a + off belongs (both kernels)
+    "scale_fwd",            # forward uses scale * (1 + 2^-8)
+    "scale_bwd",            # backward uses scale * (1 + 2^-8)
+    "bias_natural_fwd",     # forward adds the key bias in natural units to log2-unit scores
+    "bias_natural_bwd",     # backward does the same
+    "carried_l4",           # carried state loaded with l = 4 instead of 1 (lse counted twice over)
+    "dead_revive_stale_m",  # a row dead in the carried state is loaded as if its lse were 0
+    "gqa_wrong_head",       # the last query head reads K/V head (h // G + 1) mod Hkv
+    "dk_no_scale",          # dK not multiplied by scale
+    "dq_missing_key_block", # dQ misses the partial of one 128-key block
+    "dv_missing_q_block",   # dV misses the first 64-row Q block a causal key block sees (i_begin one block late)
+)
+
+
+def unit_roundoff(dtype: torch.dtype) -> float:
+    return {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}[dtype]
+
+
+def _round(x: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    return x.to(dtype).to(torch.float32)
+
+
+def _scale_log2(scale: float) -> float:
+    return float(torch.tensor(scale, dtype=torch.float32) * torch.tensor(LOG2E, dtype=torch.float32))
+
+
+def visible(sq: int, sk: int, mask, device=None, shift: int = 0, strict: bool = False):
+    """[sq, sk] bool visibility of ``mask`` (None: everything visible); ``shift`` / ``strict`` are mutant hooks."""
+    if mask is None:
+        return None
+    kind, off = mask
+    assert kind == "causal_offset", mask
+    a = torch.arange(sq, device=device).unsqueeze(1)
+    b = torch.arange(sk, device=device).unsqueeze(0)
+    return b < a + int(off) + shift if strict else b <= a + int(off) + shift
+
+
+def _kv_heads(t: torch.Tensor, H: int, mutant=None) -> torch.Tensor:
+    """K or V [B, Sk, Hkv, D] -> [B, Sk, H, D]: query head h reads K/V head h // G."""
+    Hkv = t.shape[2]
+    G = H // Hkv
+    idx = torch.arange(H, device=t.device) // G
+    if mutant == "gqa_wrong_head":
+        idx[H - 1] = (idx[H - 1] + 1) % Hkv
+    return t.index_select(2, idx)
+
+
+def _group_sum(t: torch.Tensor, Hkv: int) -> torch.Tensor:
+    B, S, H, D = t.shape
+    return t.view(B, S, Hkv, H // Hkv, D).sum(3)
+
+
+def _drop_keys(sk: int, mutant) -> list:
+    return {"drop_key_127": [127], "drop_key_128": [128], "drop_key_last": [sk - 1]}.get(mutant, [])
+
+
+def _scores_log2(q, k, scale, key_bias, mutant, side):
+    """fp32 scores in log2 units [B, H, Sq, Sk] (+ the key bias in log2 units)."""
+    if mutant == "scale_" + side:
+        scale = scale * (1 + 2.0 ** -8)
+    s = torch.einsum("bqhd,bkhd->bhqk", q.float(), k.float()) * _scale_log2(scale)
+    if key_bias is not None:
+        b = key_bias.float() * (1.0 if mutant == "bias_natural_" + side else LOG2E)
+        s = s + b.unsqueeze(2)
+    return s
+
+
+def _vis_for(sq, sk, mask, device, mutant, side):
+    shift = {"causal_plus1_" + side: 1, "causal_minus1_" + side: -1}.get(mutant, 0)
+    return visible(sq, sk, mask, device, shift=shift, strict=mutant == "strict_swap")
+
+
+def lowp_forward(q, k, v, scale, mask=None, key_bias=None, state=None, last=True, mutant=None):
+    """One forward chunk with carried state, rounded like ``fwd_chunk_kernel``.
+
+    q [B,Sq,H,D], k/v [B,Sk,Hkv,D] (16-bit); key_bias fp32 [B|1,H,Sk] or None; state ``(o_acc fp32 [B,Sq,H,D],
+    lse fp32 [B,H,Sq])`` from the previous chunk or None.  Returns ``(o, lse)``: o in the input dtype when ``last``,
+    else the fp32 normalised state the kernel leaves in o_acc.  Rows that see nothing have o = 0 and lse = -inf.
+    """
+    dtype = q.dtype
+    B, Sq, H, D = q.shape
+    Sk = k.shape[1]
+    kk, vv = _kv_heads(k, H, mutant), _kv_heads(v, H, mutant)
+    s = _scores_log2(q, kk, scale, key_bias, mutant, "fwd")
+    vis = _vis_for(Sq, Sk, mask, q.device, mutant, "fwd")
+    if vis is not None:
+        s = s.masked_fill(~vis, NEG_INF)
+    for j in _drop_keys(Sk, mutant):
+        if 0 <= j < Sk:
+            s[..., j] = NEG_INF
+    m = s.amax(-1)  # [B,H,Sq]
+    if state is not None:
+        o0 = state[0].float().permute(0, 2, 1, 3)  # [B,H,Sq,D]
+        lse0 = state[1].float()
+        alive = lse0 != NEG_INF
+        m0 = lse0 * LOG2E
+        l0 = alive.float() * (4.0 if mutant == "carried_l4" else 1.0)
+        if mutant == "dead_revive_stale_m":
+            m0 = torch.where(alive, m0, torch.zeros_like(m0))
+            l0 = torch.ones_like(l0)
+        m = torch.maximum(m, m0)
+    msafe = torch.where(m == NEG_INF, torch.zeros_like(m), m)
+    p = torch.exp2(s - msafe.unsqueeze(-1))
+    l = p.sum(-1)
+    o = torch.einsum("bhqk,bhkd->bhqd", _round(p, dtype), vv.float().permute(0, 2, 1, 3))
+    if state is not None:
+        f = torch.exp2(m0 - msafe)
+        l = l + l0 * f
+        o = o + o0 * f.unsqueeze(-1)
+    inv = torch.where(l > 0, 1.0 / l, torch.zeros_like(l))
+    o = (o * inv.unsqueeze(-1)).permute(0, 2, 1, 3).contiguous()
+    lse = torch.where(l > 0, (m + torch.log2(l)) * LN2, torch.full_like(l, NEG_INF))
+    return (o.to(dtype) if last else o), lse
+
+
+def lowp_backward(q, k, v, do, o, lse, scale, mask=None, key_bias=None, mutant=None):
+    """One backward chunk, rounded like ``delta_kernel`` + ``bwd_chunk_kernel``.
+
+    o: the 16-bit forward output, lse: the final fp32 lse (-inf: the row saw nothing, P = 0).
+    Returns fp32 ``(dq [B,Sq,H,D], dk [B,Sk,Hkv,D], dv [B,Sk,Hkv,D])`` partials of this chunk.
+    """
+    dtype = q.dtype
+    B, Sq, H, D = q.shape
+    Sk, Hkv = k.shape[1], k.shape[2]
+    kk, vv = _kv_heads(k, H, mutant), _kv_heads(v, H, mutant)
+    delta = (o.float() * do.float()).sum(-1).permute(0, 2, 1)  # [B,H,Sq]
+    s = _scores_log2(q, kk, scale, key_bias, mutant, "bwd")
+    lse2 = torch.where(lse == NEG_INF, torch.full_like(lse, float("inf")), lse.float()) * LOG2E
+    p = torch.exp2(s - lse2.unsqueeze(-1))
+    vis = _vis_for(Sq, Sk, mask, q.device, mutant, "bwd")
+    if vis is not None:
+        p = p.masked_fill(~vis, 0.0)
+    for j in _drop_keys(Sk, mutant):
+        if 0 <= j < Sk:
+            p[..., j] = 0.0
+    p_dv = _round(p, dtype)
+    if mutant == "dv_missing_q_block" and mask is not None:
+        # per 128-key block, skip the first 64-row Q block it would visit
+        off = int(mask[1])
+        for k0 in range(0, Sk, 128):
+            qb = max(0, k0 - off) // 64 * 64
+            p_dv[..., qb:qb + 64, k0:k0 + 128] = 0.0
+    dv = torch.einsum("bhqk,bqhd->bkhd", p_dv, do.float())
+    dp = torch.einsum("bqhd,bkhd->bhqk", do.float(), vv.float())
+    ds = _round(p * (dp - delta.unsqueeze(-1)), dtype)
+    ds_q = ds
+    if mutant == "dq_missing_key_block":
+        kb = 128 if Sk > 128 else 0
+        ds_q = ds.clone()
+        ds_q[..., kb:kb + 128] = 0.0
+    dq = torch.einsum("bhqk,bkhd->bqhd", ds_q, kk.float()) * scale
+    dk = torch.einsum("bhqk,bqhd->bkhd", ds, q.float()) * (1.0 if mutant == "dk_no_scale" else scale)
+    return dq, _group_sum(dk, Hkv), _group_sum(dv, Hkv)
+
+
+# --------------------------------------------------------------------------- #
+# chains of chunks: the model and the fp64 oracle side by side
+# --------------------------------------------------------------------------- #
+def lowp_chain(q, ks, vs, do, scale, masks, biases=None, mutant=None):
+    """Forward over K/V chunks ``ks[c], vs[c]`` (mask ``masks[c]``, key bias ``biases[c]``) with the fp32 state
+    carried between chunks, then the backward of every chunk against the final (O, lse).
+    Returns dict(o, lse, states=[(o_acc, lse) after each non-last chunk], dq, dk=[per chunk], dv=[per chunk])."""
+    n = len(ks)
+    biases = biases or [None] * n
+    state, states = None, []
+    for c in range(n):
+        o, lse = lowp_forward(q, ks[c], vs[c], scale, masks[c], biases[c], state, last=c == n - 1, mutant=mutant)
+        if c < n - 1:
+            state = (o, lse)
+            states.append(state)
+    dq = torch.zeros(q.shape, device=q.device, dtype=torch.float32)
+    dks, dvs = [], []
+    for c in range(n):
+        dqc, dk, dv = lowp_backward(q, ks[c], vs[c], do, o, lse, scale, masks[c], biases[c], mutant=mutant)
+        dq += dqc
+        dks.append(dk)
+        dvs.append(dv)
+    return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs)
+
+
+def oracle_chain(q, ks, vs, do, scale, masks, biases=None):
+    """The same chain in fp64 with ``oracle.attention_oracle`` (on the CPU), on the same 16-bit inputs."""
+    n = len(ks)
+    biases = biases or [None] * n
+    cpu = lambda t: None if t is None else t.detach().cpu()  # noqa: E731
+    q, do = cpu(q), cpu(do)
+    H, Hkv = q.shape[2], ks[0].shape[2]
+    kx = [_kv_heads(cpu(k), H) for k in ks]
+    vx = [_kv_heads(cpu(v), H) for v in vs]
+    modes = ["none" if m is None else m for m in masks]
+    o, lse, states = None, None, []
+    for c in range(n):
+        o, lse = orc.chunk_forward(q, kx[c], vx[c], o, lse, scale, modes[c], key_bias=cpu(biases[c]))
+        if c < n - 1:
+            states.append((o, lse))
+    delta = orc.compute_delta(o, do)
+    lse_b = torch.where(torch.isinf(lse), torch.full_like(lse, float("inf")), lse)  # dead rows: P = 0
+    dq = torch.zeros(q.shape, dtype=torch.float64)
+    dks, dvs = [], []
+    # Per gradient row, two error scales no 16-bit model run reproduces by itself:
+    # rss: the root sum of squares of the row's terms (P V for O, P dO for dV, dS K scale for dQ, dS Q scale for dK).
+    #   A 16-bit rounding moves each term by at most u/2 of itself, so where a row's terms cancel (sum_k dS = 0
+    #   exactly) or one term dominates, one model run can happen to land near the truth while the kernel does not.
+    #   delta comes from the 16-bit O, whose rounding moves delta by ~u sqrt(sum_d (O_d dO_d)^2) and every dS of the
+    #   row by P times that: in a peaky row this term, not the rounding of dS, dominates dQ and dK (for dK the
+    #   rows' shifts are added coherently, an upper bound).
+    # e32: dS = P (dP - delta) with dP from fp32 tensor-core accumulation and delta from a separate fp32 sum keeps
+    #   ~2^-23 sum_d |dO_d V_d| of rounding per element, which reaches dQ through |K| and dK through |Q|.
+    ss = dict(o=torch.zeros(q.shape[:3], dtype=torch.float64), dq=torch.zeros(q.shape[:3], dtype=torch.float64))
+    ss_dk, ss_dv, e32_dk = [], [], []
+    e32_dq = torch.zeros(q.shape[:3], dtype=torch.float64)
+    qd, dod = q.double(), do.double()
+    n2 = lambda t: t.double().pow(2).sum(-1)  # noqa: E731  [B,S,H] squared row norms
+    dd = n2(o.double() * dod).sqrt().permute(0, 2, 1)  # [B,H,Sq]
+    dq_d = torch.zeros(q.shape[:3], dtype=torch.float64)
+    for c in range(n):
+        dqc, dk, dv = orc.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, modes[c], key_bias=cpu(biases[c]))
+        dq += dqc
+        dks.append(_group_sum(dk, Hkv))
+        dvs.append(_group_sum(dv, Hkv))
+        kd, vd = kx[c].double(), vx[c].double()
+        s = torch.einsum("bqhd,bkhd->bhqk", qd, kd) * scale
+        if biases[c] is not None:
+            s = s + cpu(biases[c]).double().unsqueeze(2)
+        p = torch.exp(s - lse_b.unsqueeze(-1))
+        vis = visible(q.shape[1], kd.shape[1], masks[c])
+        if vis is not None:
+            p = p.masked_fill(~vis, 0.0)
+        ds = p * (torch.einsum("bqhd,bkhd->bhqk", dod, vd) - delta.unsqueeze(-1)) * scale
+        ss["o"] += torch.einsum("bhqk,bkh->bqh", p * p, n2(vd))
+        pd = p * dd.unsqueeze(-1) * abs(scale)  # [B,H,Sq,Sk]: the dS shift of one unit of delta rounding
+        ss["dq"] += torch.einsum("bhqk,bkh->bqh", ds * ds, n2(kd))
+        dq_d = dq_d + torch.einsum("bhqk,bkh->bqh", pd, kd.norm(dim=-1))
+        ss_dk.append(_group_sum((torch.einsum("bhqk,bqh->bkh", ds * ds, n2(qd)) +
+                                 torch.einsum("bhqk,bqh->bkh", pd, qd.norm(dim=-1)).pow(2)).unsqueeze(-1), Hkv)[..., 0])
+        ss_dv.append(_group_sum(torch.einsum("bhqk,bqh->bkh", p * p, n2(dod)).unsqueeze(-1), Hkv)[..., 0])
+        w = 2.0 ** -23 * abs(scale) * p * torch.einsum("bqhd,bkhd->bhqk", dod.abs(), vd.abs())
+        e32_dq += torch.einsum("bhqk,bkh->bqh", w, kd.norm(dim=-1))
+        e32_dk.append(_group_sum(torch.einsum("bhqk,bqh->bkh", w, qd.norm(dim=-1)).unsqueeze(-1), Hkv)[..., 0])
+    rss = dict(o=(ss["o"] + n2(o)).sqrt(), dq=(ss["dq"] + dq_d.pow(2)).sqrt(), dk=torch.cat(ss_dk, 1).sqrt(),
+               dv=torch.cat(ss_dv, 1).sqrt())
+    # the size of one key's contribution to a gradient row, before any cancellation (the comparator's floor)
+    nrm = lambda ts: max(float(t.double().norm(dim=-1).max()) for t in ts)  # noqa: E731
+    nq, ndo, nk, nv = nrm([q]), nrm([do]), nrm(kx), nrm(vx)
+    mag = dict(dq=abs(scale) * ndo * nv * nk, dk=abs(scale) * ndo * nv * nq, dv=ndo)
+    return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs, mag=mag, rss=rss,
+                e32=dict(dq=e32_dq, dk=torch.cat(e32_dk, 1)))
+
+
+def scores_absmax(q, ks, scale, masks, biases=None):
+    """[B,H,Sq]: per row, the largest ``sum_d |q_d k_d| scale + |bias|`` over the keys the row sees in any chunk --
+    the magnitude the fp32 score arithmetic works at, which bounds its rounding error."""
+    n = len(ks)
+    biases = biases or [None] * n
+    q = q.detach().cpu().double().abs()
+    H = q.shape[2]
+    out = torch.zeros(q.shape[0], H, q.shape[1], dtype=torch.float64)
+    for c in range(n):
+        k = _kv_heads(ks[c].detach().cpu(), H).double().abs()
+        a = torch.einsum("bqhd,bkhd->bhqk", q, k) * abs(scale)
+        if biases[c] is not None:
+            bb = biases[c].detach().cpu().double().abs()
+            a = a + torch.where(torch.isinf(bb), torch.zeros_like(bb), bb).unsqueeze(2)
+        vis = visible(q.shape[1], k.shape[1], masks[c])
+        if vis is not None:
+            a = a.masked_fill(~vis, 0.0)
+        if biases[c] is not None:
+            a = a.masked_fill(torch.isinf(biases[c].detach().cpu()).unsqueeze(2).expand_as(a), 0.0)
+        out = torch.maximum(out, a.amax(-1))
+    return out
+
+
+# --------------------------------------------------------------------------- #
+# the comparator
+# --------------------------------------------------------------------------- #
+# Global: max|got - ref| <= A * max|model - ref| + FLOOR * mag (+ max(extra), below).
+# Per (b, s, h) row of length D: |got - ref| <= B * |model - ref| + C * u * rss + FLOOR * mag + extra, where rss is
+# the root sum of squares of the row's terms (default |ref|) and extra (dQ, dK) the fp32 bound e32, both from
+# ``oracle_chain``; the global bound adds max(extra).
+# mag is the size of one unit of the output before any cancellation (default: the largest row norm of ref; for the
+# gradients ``oracle_chain`` derives it from the input norms): where the exact result cancels to zero -- dQ and dK
+# of a row or key with a single visible partner, whose dS = P (dP - delta) is exactly zero -- the kernels are left
+# with the fp32 rounding of dP - delta, which no 16-bit model reproduces.
+# lse: |got - ref| <= LSE_A * 2^-23 * (|ref| + scores_absmax), -inf exactly where the reference is -inf.
+# Set from the H100 calibration of tests/test_gpu_tile_edges.py so that the kernels use at most half of every bound
+# (WORST; test_report_worst_ratios there prints it).  The same constants serve bf16 and fp16: u carries the dtype.
+A = 3.0
+B = 4.0
+C = 2.0
+FLOOR = 2.0 ** -20
+LSE_A = 4.0
+
+# worst bound usage seen in this process, error / bound (the check passes at <= 1):
+# {(output, dtype name): ((global usage, case), (worst row usage, case))}
+WORST: dict = {}
+
+
+def _note(name, dt, glob, row):
+    key = (name.split("[")[0], dt)
+    case = name[name.find("[") + 1:-1] if "[" in name else name
+    g0, r0 = WORST.get(key, ((0.0, ""), (0.0, "")))
+    WORST[key] = (max(g0, (glob, case)), max(r0, (row, case)))
+
+
+def assert_within_model(name, got, ref, model, dtype, mag=None, extra=None, rss=None):
+    """``got`` (kernel), ``ref`` (fp64 oracle) and ``model`` (lowp_*) of one output [B,S,H,D]; see the constants."""
+    got, ref, model = (t.detach().double().cpu() for t in (got, ref, model))
+    assert got.shape == ref.shape == model.shape, (name, got.shape, ref.shape, model.shape)
+    assert torch.isfinite(got).all(), f"{name}: {int((~torch.isfinite(got)).sum())} non-finite values"
+    u = unit_roundoff(dtype)
+    err, merr = (got - ref).abs(), (model - ref).abs()
+    en, mn, rn = (got - ref).norm(dim=-1), (model - ref).norm(dim=-1), ref.norm(dim=-1)
+    if mag is None:
+        mag = float(rn.max()) if rn.numel() else 0.0
+    floor = FLOOR * mag
+    extra = torch.zeros_like(en) if extra is None else extra.detach().double().cpu()
+    rss = rn if rss is None else rss.detach().double().cpu()
+    tiny = torch.finfo(torch.float64).tiny
+    g_err, g_model = float(err.max()), float(merr.max())
+    g_bound = A * g_model + floor + float(extra.max())
+    g_use = g_err / max(g_bound, tiny) if g_err > 0 else 0.0
+    row_bound = (B * mn + C * u * rss + floor + extra).clamp(min=tiny)
+    row_use = torch.where(en > 0, en / row_bound, torch.zeros_like(en))
+    _note(name, str(dtype).replace("torch.", ""), g_use, float(row_use.max()))
+    assert g_use <= 1.0, (
+        f"{name}: max|got-ref| {g_err:.3e} > {A} x max|model-ref| {g_model:.3e} + floor {floor:.1e} + "
+        f"fp32 term {float(extra.max()):.1e} "
+        f"(at {tuple(int(i) for i in torch.unravel_index(err.argmax(), err.shape))})")
+    bad = row_use > 1.0
+    if bad.any():
+        idx = bad.nonzero()
+        worst = tuple(int(i) for i in torch.unravel_index(row_use.argmax(), row_use.shape))
+        raise AssertionError(
+            f"{name}: {int(bad.sum())} of {bad.numel()} (b, s, h) rows outside the model bound, e.g. rows "
+            f"(b, s, h) {[tuple(r) for r in idx[:8].tolist()]}; worst {worst}: |got-ref| {float(en[worst]):.3e}, "
+            f"|model-ref| {float(mn[worst]):.3e}, |ref| {float(rn[worst]):.3e}")
+
+
+def assert_lse(name, got, ref, absmax):
+    """lse [B,H,S] (fp32 kernel vs fp64 oracle); ``absmax`` from ``scores_absmax``."""
+    got, ref, absmax = (t.detach().double().cpu() for t in (got, ref, absmax))
+    dead = torch.isinf(ref) & (ref < 0)
+    assert not torch.isnan(got).any(), f"{name}: NaN in lse"
+    assert torch.equal(torch.isinf(got) & (got < 0), dead), (
+        f"{name}: lse is -inf at {int((torch.isinf(got) & (got < 0)).sum())} rows, the oracle at {int(dead.sum())}")
+    g, r, a = got[~dead], ref[~dead], absmax[~dead]
+    if g.numel() == 0:
+        return
+    tol = 2.0 ** -23 * (r.abs() + a)
+    ratio = float(((g - r).abs() / tol.clamp(min=torch.finfo(torch.float64).tiny)).max())
+    _note(name, "fp32", ratio / LSE_A, ratio / LSE_A)
+    assert ratio <= LSE_A, f"{name}: |lse - ref| reaches {ratio:.2f} x 2^-23 (|ref| + scores_absmax), limit {LSE_A}"
+
+
+def uniform_closed_form(vs, masks, sq):
+    """q = 0 and no bias: every visible key has the same score, so O is the mean of the visible V rows and
+    lse = log(#visible).  vs: the chunks' V [B,Sk,H,D] (already at the query heads); returns fp64
+    (o [B,Sq,H,D], lse [Sq])."""
+    num, n = 0.0, torch.zeros(sq, dtype=torch.float64)
+    for v, m in zip(vs, masks):
+        v = v.detach().cpu().double()
+        vis = visible(sq, v.shape[1], m)
+        w = torch.ones(sq, v.shape[1], dtype=torch.float64) if vis is None else vis.double()
+        num = num + torch.einsum("qk,bkhd->bqhd", w, v)
+        n += w.sum(-1)
+    o = num / n.clamp(min=1).view(1, sq, 1, 1)
+    lse = torch.where(n > 0, n.log(), torch.full_like(n, NEG_INF))
+    return o, lse
+
+
+def assert_chain_within_model(name, got, ref, model, dtype, absmax_prefix):
+    """Every output of a chain (``lowp_chain`` / ``oracle_chain`` dicts): the fp32 state after each non-last chunk,
+    O, lse, dQ and the per-chunk dK, dV.  ``absmax_prefix[c]``: ``scores_absmax`` over chunks 0..c."""
+    for c, (g, r, m) in enumerate(zip(got["states"], ref["states"], model["states"])):
+        assert_within_model(f"o_acc[{name} chunk {c}]", g[0], r[0], m[0], dtype)
+        assert_lse(f"lse_state[{name} chunk {c}]", g[1], r[1], absmax_prefix[c])
+    r = ref
+    assert_within_model(f"o[{name}]", got["o"], r["o"], model["o"], dtype, rss=r["rss"]["o"])
+    assert_lse(f"lse[{name}]", got["lse"], r["lse"], absmax_prefix[-1])
+    assert_within_model(f"dq[{name}]", got["dq"], r["dq"], model["dq"], dtype, r["mag"]["dq"], r["e32"]["dq"],
+                        r["rss"]["dq"])
+    cat = lambda d, k: torch.cat([t.detach().cpu().double() for t in d[k]], dim=1)  # noqa: E731
+    assert_within_model(f"dk[{name}]", cat(got, "dk"), cat(r, "dk"), cat(model, "dk"), dtype, r["mag"]["dk"],
+                        r["e32"]["dk"], r["rss"]["dk"])
+    assert_within_model(f"dv[{name}]", cat(got, "dv"), cat(r, "dv"), cat(model, "dv"), dtype, r["mag"]["dv"],
+                        rss=r["rss"]["dv"])
+
+
+# --------------------------------------------------------------------------- #
+# the tile-edge sweep (tests/test_gpu_tile_edges.py runs it on the kernels, tests/test_lowp_model.py on the model)
+# --------------------------------------------------------------------------- #
+# Forward tiles are 128 Q rows x 128 keys; backward tiles 128 keys x 64 Q rows.  A case: Sq query rows against a
+# chain of K/V chunks (Sk, causal offset or None), the softmax scale ("d": D^-0.5), a score distribution, a key
+# bias kind, batch / heads, the layout the kernels see ("flash" [B,S,H,D], "normal" [B,H,S,D], "bstride": x[::2] of
+# a batch twice as large) and an input amplitude.
+_DT = (torch.bfloat16, torch.float16)
+_OFFSETS = lambda sq, sk: [-sk, -129, -128, -65, -64, -63, -1, 0, 1, 63, 64, 65, 127, 128, 129, sk - sq, sk]  # noqa
+
+
+def _case(sq, chunks, D=128, dtype=torch.bfloat16, scale="d", dist="randn", bias=None, B=1, H=2, Hkv=None,
+          layout="flash", amp=1.0, tag=""):
+    if len(chunks) > 3:  # long chains: number of chunks, total keys, offset of the first chunk
+        ch = f"{len(chunks)}chunks{sum(sk for sk, _ in chunks)}" + ("" if chunks[0][1] is None else f"@{chunks[0][1]}")
+    else:
+        ch = "+".join(f"{sk}" + ("" if off is None else f"@{off}") for sk, off in chunks)
+    name = f"{tag}q{sq}_k{ch}_d{D}_{'bf16' if dtype == torch.bfloat16 else 'fp16'}_s{scale}_{dist}"
+    if bias:
+        name += f"_bias-{bias}"
+    if B != 1 or H != 2 or Hkv:
+        name += f"_B{B}H{H}kv{Hkv or H}"
+    if layout != "flash":
+        name += f"_{layout}"
+    if amp != 1.0:
+        name += f"_x{amp:g}"
+    return dict(id=name, sq=sq, chunks=list(chunks), D=D, dtype=dtype, scale=scale, dist=dist, bias=bias, B=B, H=H,
+                Hkv=Hkv or H, layout=layout, amp=amp)
+
+
+def _sweep():
+    cases = []
+    # every Sq in {1, 63, 64, 65, 127, 128, 129, 255, 257, 383} and Sk in {1, 2, 63, 127, 128, 129, 255, 256, 257, 513}
+    pairs = [(1, 513), (63, 129), (64, 1), (65, 127), (127, 2), (128, 257), (129, 63), (255, 128), (257, 255),
+             (383, 256), (1, 1), (129, 129), (257, 513), (65, 2)]
+    for i, (sq, sk) in enumerate(pairs):
+        for j, (D, dt) in enumerate([(64, _DT[0]), (64, _DT[1]), (128, _DT[0]), (128, _DT[1])]):
+            cases.append(_case(sq, [(sk, None)], D, dt))
+        D, dt = [(64, _DT[0]), (128, _DT[1]), (128, _DT[0]), (64, _DT[1])][i % 4]
+        cases.append(_case(sq, [(sk, sk - sq)], D, dt))  # bottom-right causal
+    # causal offsets one key either side of every forward (128) and backward (64) tile edge, both signs
+    for sq, sk in [(255, 257), (129, 513)]:
+        for i, off in enumerate(_OFFSETS(sq, sk)):
+            D, dt = [(128, _DT[0]), (64, _DT[1]), (64, _DT[0]), (128, _DT[1])][i % 4]
+            cases.append(_case(sq, [(sk, off)], D, dt))
+    # softmax scales x score distributions
+    for i, scale in enumerate([0.01, "d", 0.3, 1.0]):
+        for j, dist in enumerate(["randn", "rising", "last_tile", "zero_q"]):
+            D, dt = [(128, _DT[0]), (64, _DT[1]), (128, _DT[1]), (64, _DT[0])][(i + j) % 4]
+            sq, sk = (129, 257) if j % 2 == 0 else (255, 513)
+            off = None if (i + j) % 2 == 0 else sk - sq
+            cases.append(_case(sq, [(sk, off)], D, dt, scale=scale, dist=dist))
+    # carried state: chains of 2, 5 and 16 chunks (views of one causal problem: offset = q_start - k_start)
+    def causal_chain(sq, sizes, q_start):
+        out, k0 = [], 0
+        for sk in sizes:
+            out.append((sk, q_start - k0))
+            k0 += sk
+        return out
+    for D, dt in [(128, _DT[0]), (64, _DT[1])]:
+        cases.append(_case(129, [(128, None), (129, None)], D, dt))
+        cases.append(_case(129, causal_chain(129, [128, 129], 128), D, dt))
+        cases.append(_case(255, [(63, None), (127, None), (1, None), (129, None), (255, None)], D, dt))
+        cases.append(_case(255, causal_chain(255, [128] * 5, 640 - 255), D, dt))
+        cases.append(_case(129, [(64, None)] * 16, D, dt))
+        cases.append(_case(129, causal_chain(129, [64] * 16, 1024 - 129), D, dt))
+        # the first chunk leaves every row (offset <= -Sq) or the first 64 rows dead; later chunks revive them
+        cases.append(_case(129, [(128, -129), (128, 128), (129, 0)], D, dt, tag="dead1st_"))
+        cases.append(_case(129, [(128, -64), (257, 200)], D, dt, tag="dead1st_"))
+        cases.append(_case(65, [(1, -65), (127, -1), (63, 64), (2, 70), (255, 127)], D, dt, tag="dead1st_"))
+    cases.append(_case(257, causal_chain(257, [64] * 16, 1024 - 257), 128, _DT[0], scale=1.0, dist="rising"))
+    # key bias
+    for D, dt in [(128, _DT[0]), (64, _DT[1])]:
+        cases.append(_case(129, [(257, None)], D, dt, bias="randn"))
+        cases.append(_case(129, [(257, 128)], D, dt, bias="randn"))
+        cases.append(_case(127, [(383, None)], D, dt, bias="tile_inf"))
+        cases.append(_case(255, [(257, None)], D, dt, bias="edge_inf"))
+        cases.append(_case(129, [(257, 128)], D, dt, bias="edge_inf"))
+        cases.append(_case(129, [(255, None)], D, dt, bias="bcast", B=2))
+        cases.append(_case(129, [(129, 0)], D, dt, bias="dead_rows"))
+        cases.append(_case(65, [(128, None)], D, dt, bias="head_dead"))
+        cases.append(_case(129, [(128, -64), (129, 64)], D, dt, bias="randn", tag="chain_"))
+    # layouts and grouped-query attention
+    for D, dt in [(128, _DT[1]), (64, _DT[0])]:
+        cases.append(_case(129, [(257, 128)], D, dt, B=2, layout="bstride"))
+        cases.append(_case(255, [(129, None)], D, dt, B=2, layout="bstride", bias="randn"))
+        cases.append(_case(129, [(257, 65)], D, dt, layout="normal"))
+        cases.append(_case(65, [(128, None), (63, 64)], D, dt, layout="normal"))
+        for hkv in (4, 2, 1):
+            cases.append(_case(129, [(257, 127)], D, dt, H=4, Hkv=hkv))
+        cases.append(_case(255, [(129, -63)], D, dt, H=4, Hkv=2, bias="randn", layout="normal"))
+    # fp16 range: inputs x 4
+    for D in (64, 128):
+        cases.append(_case(129, [(513, None)], D, _DT[1], amp=4.0))
+        cases.append(_case(255, [(257, 1)], D, _DT[1], scale=1.0, amp=4.0))
+        cases.append(_case(129, causal_chain(129, [128, 129], 128), D, _DT[1], amp=4.0))
+    ids = [c["id"] for c in cases]
+    assert len(ids) == len(set(ids)), "duplicate case ids"
+    return cases
+
+
+SWEEP = _sweep()
+
+
+def make_inputs(case, device="cpu"):
+    """The case's 16-bit inputs in the logical flash layout, on ``device``:
+    dict(q, ks, vs, do, scale, masks, biases)."""
+    import zlib
+    g = torch.Generator().manual_seed(zlib.crc32(case["id"].encode()))
+    B, H, Hkv, D, sq, dt, amp = case["B"], case["H"], case["Hkv"], case["D"], case["sq"], case["dtype"], case["amp"]
+    rn = lambda *s: torch.randn(*s, generator=g, dtype=torch.float32)  # noqa: E731
+    e = torch.ones(D) / D ** 0.5  # a direction every query shares with the keys it favours
+    q = rn(B, sq, H, D)
+    do = rn(B, sq, H, D)
+    ks, vs, k0 = [], [], 0
+    n_total = sum(sk for sk, _ in case["chunks"])
+    for sk, _ in case["chunks"]:
+        k, v = rn(B, sk, Hkv, D), rn(B, sk, Hkv, D)
+        pos = torch.arange(k0, k0 + sk, dtype=torch.float32)
+        if case["dist"] == "rising":  # every 128-key tile scores higher than the one before
+            k = 0.5 * k + ((pos // 128 + 1) * 1.0).view(1, sk, 1, 1) * e
+        elif case["dist"] == "last_tile":  # the row maximum sits in the last, ragged tile of the last chunk
+            last = pos >= (n_total - 1) // 128 * 128
+            k = 0.3 * k + last.float().view(1, sk, 1, 1) * 3.0 * e
+        ks.append(k)
+        vs.append(v)
+        k0 += sk
+    if case["dist"] == "rising":
+        q = 0.5 * q + 4.0 * e
+    elif case["dist"] == "last_tile":
+        q = 0.3 * q + 3.0 * e
+    elif case["dist"] == "zero_q":
+        q = torch.zeros_like(q)
+    biases = []
+    for sk, _ in case["chunks"]:
+        kind = case["bias"]
+        if kind is None:
+            biases.append(None)
+            continue
+        b = 2.0 * rn(1 if kind == "bcast" else B, H, sk)
+        if kind == "tile_inf":
+            b[..., 128:256] = NEG_INF
+        elif kind == "edge_inf":
+            for j in (127, 128, sk - 1):
+                if j < sk:
+                    b[..., j] = NEG_INF
+        elif kind == "dead_rows":  # with the causal diagonal: rows 0..63 see only these keys
+            b[..., :64] = NEG_INF
+        elif kind == "head_dead":  # every key of the last query head
+            b[:, -1] = NEG_INF
+        if kind == "bcast":
+            b = b.expand(B, H, sk)
+        biases.append(b.to(device))
+    scale = D ** -0.5 if case["scale"] == "d" else float(case["scale"])
+    cvt = lambda t: (amp * t).to(dt).to(device)  # noqa: E731
+    return dict(q=cvt(q), ks=[cvt(k) for k in ks], vs=[cvt(v) for v in vs], do=cvt(do), scale=scale,
+                masks=[None if off is None else ("causal_offset", off) for _, off in case["chunks"]], biases=biases)
