@@ -430,6 +430,24 @@ def assert_chain_within_model(name, got, ref, model, dtype, absmax_prefix):
                         rss=r["rss"]["dv"])
 
 
+def assert_api_within_model(name, got, ref, model, dtype, absmax=None):
+    """What the public API returns for one call -- ``got``: dict(o, dq, dk, dv) [B,S,H,D] and, checked when
+    ``absmax`` (``scores_absmax``) is given, lse [B,H,S] -- against ``oracle_chain`` / ``lowp_chain`` of the same
+    problem.  The API returns 16-bit gradients, so the model's fp32 gradients are rounded to 16 bit first."""
+    rnd = lambda t: t.to(dtype).float()  # noqa: E731
+    cat = lambda d, k: torch.cat([t.detach().cpu().double() for t in d[k]], dim=1)  # noqa: E731
+    r = ref
+    assert_within_model(f"o[{name}]", got["o"], r["o"], model["o"], dtype, rss=r["rss"]["o"])
+    if absmax is not None:
+        assert_lse(f"lse[{name}]", got["lse"], r["lse"], absmax)
+    assert_within_model(f"dq[{name}]", got["dq"], r["dq"], rnd(model["dq"]), dtype, r["mag"]["dq"], r["e32"]["dq"],
+                        r["rss"]["dq"])
+    assert_within_model(f"dk[{name}]", got["dk"], cat(r, "dk"), rnd(cat(model, "dk")), dtype, r["mag"]["dk"],
+                        r["e32"]["dk"], r["rss"]["dk"])
+    assert_within_model(f"dv[{name}]", got["dv"], cat(r, "dv"), rnd(cat(model, "dv")), dtype, r["mag"]["dv"],
+                        rss=r["rss"]["dv"])
+
+
 # --------------------------------------------------------------------------- #
 # the tile-edge sweep (tests/test_gpu_tile_edges.py runs it on the kernels, tests/test_lowp_model.py on the model)
 # --------------------------------------------------------------------------- #

@@ -142,15 +142,7 @@ def test_public_api_softmax_scale(monkeypatch, striped, causal, scale, D, dtype,
     model = lm.lowp_chain(*args)
     ref = lm.oracle_chain(*args)
     name = f"{case['id']}_{'striped' if striped else 'contiguous'}"
-    rnd = lambda t: t.to(dtype).float()  # noqa: E731  (the API returns 16-bit gradients)
-    r = ref
-    lm.assert_within_model(f"o[{name}]", o, r["o"], model["o"], dtype, rss=r["rss"]["o"])
-    lm.assert_within_model(f"dq[{name}]", dq, r["dq"], rnd(model["dq"]), dtype, r["mag"]["dq"], r["e32"]["dq"],
-                           r["rss"]["dq"])
-    lm.assert_within_model(f"dk[{name}]", dk, r["dk"][0], rnd(model["dk"][0]), dtype, r["mag"]["dk"], r["e32"]["dk"],
-                           r["rss"]["dk"])
-    lm.assert_within_model(f"dv[{name}]", dv, r["dv"][0], rnd(model["dv"][0]), dtype, r["mag"]["dv"],
-                           rss=r["rss"]["dv"])
+    lm.assert_api_within_model(name, dict(o=o, dq=dq, dk=dk, dv=dv), ref, model, dtype)
 
 
 def test_report_worst_ratios():

@@ -8,92 +8,19 @@ reference's protocol, test/test_burst.py:159-219).  With grouped-query K/V
 group, and each forward hop must carry 1/G of the bytes of the same call with
 MHA K/V."""
 import os
-import socket
 import sys
 
 import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
+
+from ring_harness import double_group, install_staged_transport, spawn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _install_deferred_transport():
-    """Make the CPU transport behave like the asynchronous GPU one, to catch buffer hazards gloo's eager
-    transfers hide: between ``post`` and ``wait`` a hop's destinations hold garbage (poisoned with NaN here, so
-    any read before ``wait`` shows up in the results) and its sources must not change (snapshotted at ``post``
-    and compared at ``wait``, which is when the transfer actually runs)."""
-    from burst_attn import comm
-
-    eager_commit = comm.Ring._commit_torch
-    plain_empty = comm.Ring.empty
-
-    def empty(self, shape, dtype, device):
-        t = plain_empty(self, shape, dtype, device)
-        self.__dict__.setdefault("_owned", set()).add(t.data_ptr())
-        return t
-
-    comm.Ring.empty = empty
-
-    def commit(self, srcs, dsts):
-        assert not getattr(self, "_deferred", None), "two hops in flight on one ring"
-        if self.transport == "ce":  # copy-engine rings can only receive into buffers carved from their arena
-            assert all(d.data_ptr() in getattr(self, "_owned", ()) for d in dsts), \
-                "a hop destination was not allocated through Ring.empty / empty_like"
-        self._deferred = (srcs, dsts, [s.clone() for s in srcs])
-        for d in dsts:
-            d.fill_(float("nan"))
-        return ["deferred"]
-
-    def wait(self, force_wait_inter=False):
-        for r in self._reqs:
-            assert r == "deferred"
-            srcs, dsts, snap = self._deferred
-            self._deferred = None
-            for s, c in zip(srcs, snap):
-                assert torch.equal(s, c), "a hop's source was modified between post and wait"
-            for q in eager_commit(self, srcs, dsts):
-                q.wait()
-        self._reqs = []
-
-    comm.Ring._commit_torch = commit
-    comm.Ring.wait = wait
-
-
 HQ = 4
 HKV_CASES = (2, 1)  # grouped-query K/V: G = 2 (GQA) and G = Hq (MQA)
-
-
-def _double_group(rank, world, intra, dq_groups):
-    """Hierarchical ring: nodes of `intra` consecutive ranks (reference test/test_burst.py:120-156)."""
-    from burst_attn.burst_attn_interface import _Topology, get_partition_id
-    from oracle import attention_oracle as orc
-    os.environ["BA_DOUBLE_RING"] = "1"
-    rows = [list(range(n * intra, (n + 1) * intra)) for n in range(world // intra)]
-    cols = [list(c) for c in zip(*rows)]
-    mk = lambda ranks: dist.new_subgroups_by_enumeration(ranks, backend="gloo")[0]  # noqa: E731
-    double_group = [mk(rows), mk(cols)]
-    if dq_groups:
-        double_group = [(double_group[0], mk(rows)), (double_group[1], mk(cols))]
-    topo = _Topology(None, double_group)
-    assert topo.hier and (topo.L, topo.M) == (intra, world // intra)
-    plain = [g[0] if isinstance(g, tuple) else g for g in double_group]
-    seen = sorted(get_partition_id(plain, r) for r in range(1, world + 1))
-    assert seen == list(range(world)), seen  # every shard is visited exactly once
-    assert get_partition_id(plain, 1) == rank
-    for r in range(1, world + 1):  # the oracle's restatement is pinned to the reference (tests/golden)
-        assert get_partition_id(plain, r) == orc.get_partition_id_double(r, rank % intra, rank // intra, intra,
-                                                                        world // intra)
-    return double_group
 
 
 def _check(ops, rank, world, case, seq_dim, hq, hkv, double_group=(None, None)):
@@ -159,48 +86,25 @@ def _check(ops, rank, world, case, seq_dim, hq, hkv, double_group=(None, None)):
         assert nf == world and nb == world, (nf, nb)
 
 
-def _worker(rank, world, port, errq, case, seq_dim, intra, dq_groups, gqa):
-    try:
-        for p in (ROOT, os.path.join(ROOT, "burst-attention_b200"), os.path.join(ROOT, "tests")):
-            if p not in sys.path:
-                sys.path.insert(0, p)
-        os.environ["MASTER_ADDR"] = "127.0.0.1"
-        os.environ["MASTER_PORT"] = str(port)
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        from burst_attn import chunk_ops
-        from oracle_ops import OracleOps
-        ops = OracleOps()
-        chunk_ops._set_ops_for_testing(ops)
-        if os.environ.get("BA_TEST_DEFERRED"):
-            _install_deferred_transport()
-        double_group = _double_group(rank, world, intra, dq_groups) if intra else (None, None)
-        if not (case != "none" and seq_dim == 2):  # reference asserts causal needs flash == "cuda"
-            for hq, hkv in ([(HQ, h) for h in HKV_CASES] if gqa else [(3, 3)]):
-                _check(ops, rank, world, case, seq_dim, hq, hkv, double_group)
-        dist.barrier()
-        dist.destroy_process_group()
-    except Exception as e:  # noqa: BLE001
-        import traceback
-        errq.put(f"rank {rank}: {type(e).__name__}: {e}\n{traceback.format_exc()}")
-        raise
+def _worker(rank, world, port, case, seq_dim, intra, dq_groups, gqa):
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from burst_attn import chunk_ops
+    from oracle_ops import OracleOps
+    ops = OracleOps()
+    chunk_ops._set_ops_for_testing(ops)
+    if os.environ.get("BA_TEST_DEFERRED"):
+        install_staged_transport()
+    dg = double_group(rank, world, intra, dq_groups) if intra else (None, None)
+    if not (case != "none" and seq_dim == 2):  # reference asserts causal needs flash == "cuda"
+        for hq, hkv in ([(HQ, h) for h in HKV_CASES] if gqa else [(3, 3)]):
+            _check(ops, rank, world, case, seq_dim, hq, hkv, dg)
+    dist.barrier()
+    dist.destroy_process_group()
 
 
 def _spawn(world, case, seq_dim=1, intra=0, dq_groups=False, gqa=False):
     """Run _worker on `world` gloo ranks and fail with every rank's traceback."""
-    ctx = mp.get_context("spawn")
-    errq = ctx.SimpleQueue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, errq, case, seq_dim, intra, dq_groups, gqa))
-             for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(240)
-    errs = []
-    while not errq.empty():
-        errs.append(errq.get())
-    assert not errs, "\n".join(errs)
-    assert all(p.exitcode == 0 for p in procs), [p.exitcode for p in procs]
+    spawn(_worker, world, (case, seq_dim, intra, dq_groups, gqa), timeout=240)
 
 
 @pytest.mark.parametrize("world", [2, 4])
@@ -225,7 +129,7 @@ def test_double_ring_matches_dense(world, intra, case, dq_groups):
                                               (4, 2, "zigzag"), (6, 2, "striped"), (6, 3, "none")])
 def test_no_buffer_hazards_with_asynchronous_transport(world, intra, case, monkeypatch):
     """Flat and hierarchical rings under a transport that only moves data at ``wait`` and poisons the
-    destinations at ``post`` (see _install_deferred_transport): what the side-stream transport does on GPUs."""
+    destinations at ``post`` (see ring_harness.install_staged_transport): what the side-stream transport does on GPUs."""
     monkeypatch.setenv("BA_TEST_DEFERRED", "1")
     monkeypatch.setenv("BA_RING_TRANSPORT", "ce")  # CPU tensors still travel over gloo; turns on the arena check
     _spawn(world, case, intra=intra)
