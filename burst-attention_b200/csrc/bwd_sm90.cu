@@ -28,6 +28,9 @@
 // The packed A operands (P^T for dV, dS^T for dK) stay untouched until the wait that retires their group.
 // smem (D = 128): K 32K, V 32K, Q 2x16K, dO 2x16K, dS^T 2x16K, dQ staging 16K per reducing warpgroup (single-
 // buffered: its next write waits for the previous reduce to have read it), row statistics 1K.
+// The dQ staging of a warpgroup is two [64 rows][32 fp32] SW128 boxes, one reduce-add each; lanes with odd row
+// index store their 8-column chunks in a permuted order, so every STS.64 of the staging is conflict-free (2
+// wavefronts; the bank arithmetic is next to the stores).
 #include <math.h>
 #include <stdlib.h>
 
@@ -84,16 +87,18 @@ struct BwdLayout {
   static constexpr int kBoxes = kD / 64;
   static constexpr int kBoxKV = kBwdN * 128;  // 16 KiB: [128 keys][64 cols] SW128 box
   static constexpr int kBoxQ = kBwdM * 128;   // 8 KiB: [64 rows][64 cols] SW128 box
+  static constexpr int kBoxDQ = kBwdM * 128;  // 8 KiB: [64 rows][32 fp32 cols] SW128 box
   static constexpr int kOffK = 0;
   static constexpr int kOffV = kOffK + kBoxes * kBoxKV;
   static constexpr int kOffQ = kOffV + kBoxes * kBoxKV;     // 2 stages
   static constexpr int kOffDO = kOffQ + 2 * kBoxes * kBoxQ;  // 2 stages
   static constexpr int kOffDS = kOffDO + 2 * kBoxes * kBoxQ; // 2 x [128 keys][64 q] SW128
-  static constexpr int kOffDQ = kOffDS + 2 * kBwdN * 128;    // per reducing warpgroup [64 rows][64] fp32
-  static constexpr int kOffStat = kOffDQ + kBoxes * kBwdM * 64 * 4;  // 2 stages x [lse2 | delta] x 64 fp32
+  static constexpr int kOffDQ = kOffDS + 2 * kBwdN * 128;    // per reducing warpgroup 2 dQ boxes (64 columns)
+  static constexpr int kOffStat = kOffDQ + kBoxes * 2 * kBoxDQ;  // 2 stages x [lse2 | delta] x 64 fp32
   static constexpr int kOffBar = kOffStat + 2 * 2 * kBwdM * 4;
   static constexpr int kSmemBytes = kOffBar + 64;  // no align slack: the dynamic smem base is checked to be 1 KiB aligned
   static_assert(kSmemBytes <= 232448, "backward kernel exceeds 227 KiB of shared memory");
+  static_assert(kOffDQ % 1024 == 0, "SW128 dQ staging boxes need 1 KiB alignment");
 };
 
 template <bool kBF16, int kD>
@@ -105,7 +110,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();  // SWIZZLE_128B atoms need a 1 KiB-aligned base
   using L = BwdLayout<kD>;
-  constexpr int kBoxes = L::kBoxes, kBoxKV = L::kBoxKV, kBoxQ = L::kBoxQ, kAcc = kD / 2;
+  constexpr int kBoxes = L::kBoxes, kBoxKV = L::kBoxKV, kBoxQ = L::kBoxQ, kDQBox = L::kBoxDQ, kAcc = kD / 2;
   constexpr int kQStageB = kBoxes * kBoxQ;
   float* sStat = reinterpret_cast<float*>(smem + L::kOffStat);
   BwdBarriers* bars = reinterpret_cast<BwdBarriers*>(smem + L::kOffBar);
@@ -213,7 +218,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 
   const uint32_t sK = smem_u32(smem + L::kOffK), sV = smem_u32(smem + L::kOffV);
   const uint32_t kw = wg * 64 * 128;  // this group's 64 key rows inside every K / V box
-  float* sDQ = reinterpret_cast<float*>(smem + L::kOffDQ) + wg * kBwdM * 64;
+  uint8_t* sDQ = smem + L::kOffDQ + wg * 2 * kDQBox;
   mbar_wait(&bars->kv_full, 0);
   int it = 0, h = h0;  // Q block (relative to i_begin) and query head of this step
   for (int step = 0; step < n_steps; ++step) {
@@ -350,12 +355,28 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const uint32_t bar_id = 2 + wg;
       if (tid == 0) tma_store_wait_read<0>();  // the previous reduce has finished reading the staging tile
       named_bar_sync(bar_id, 128);
+      // This thread holds dQ rows 16 w + g + 8 r (row % 8 = g) at columns 8 c + 2 t, 8 c + 2 t + 1.  Column 8 c + 2 t
+      // lies in box c / 4, 16-byte chunk j = 2 (c % 4) + t / 2 of its row, at byte 8 (t % 2) of the chunk; SW128
+      // stores chunk j at j ^ g.  Rows are 128 bytes, so the bank of a store depends on that chunk only, and one
+      // STS.64 of 16 lanes (g = 0..3 or 4..7, t = 0..3) needs 8 distinct chunks to be a single wavefront.  Storing
+      // every thread's chunk c = k at iteration k gives chunks {2 (k % 4), 2 (k % 4) + 1} ^ g: rows g and g ^ 1 meet,
+      // 2 wavefronts per half-warp.  A lane with odd g therefore stores c = k ^ 2 instead: its chunk is
+      // 2 (k % 4) ^ x with x = 4 (g % 2) ^ g ^ t / 2, and x takes all 8 values over the 16 lanes of either half-warp
+      // (g = 0..3: {0,1} {5,4} {2,3} {7,6}; g = 4..7: {4,5} {1,0} {6,7} {3,2}), so every STS.64 is 2 wavefronts, one
+      // per half-warp.  c = k ^ 2 (g % 2) runs over 0..7 once, so each of the 64 x 32 float2 slots is written once.
+      // The value is a register select between dq of chunks k and k ^ 2 (no dynamic register index).
+      const bool odd = g & 1;
+      const int x = (odd ? 4 : 0) ^ g ^ (t >> 1);
+      uint8_t* row = sDQ + (16 * w + g) * 128 + 8 * (t & 1);
 #pragma unroll
-      for (int c = 0; c < 8; ++c)
+      for (int k = 0; k < 8; ++k)
 #pragma unroll
-        for (int r = 0; r < 2; ++r)
-          *reinterpret_cast<float2*>(sDQ + (16 * w + g + 8 * r) * 64 + 8 * c + 2 * t) =
-              make_float2(dq[4 * c + 2 * r] * p.scale, dq[4 * c + 2 * r + 1] * p.scale);
+        for (int r = 0; r < 2; ++r) {
+          const int e = 4 * k + 2 * r, e2 = 4 * (k ^ 2) + 2 * r;
+          const float v0 = odd ? dq[e2] : dq[e], v1 = odd ? dq[e2 + 1] : dq[e + 1];
+          *reinterpret_cast<float2*>(row + (k >> 2) * kDQBox + r * 8 * 128 + ((2 * (k & 3) ^ x) << 4)) =
+              make_float2(v0 * p.scale, v1 * p.scale);
+        }
       fence_proxy_async_smem();
       named_bar_sync(bar_id, 128);
       if (tid == 0) {
@@ -371,7 +392,8 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
           while (ld_acquire_gpu(turn) != my_turn) __nanosleep(64);
         }
         tma_reduce_add_4d(&tmDQ, sDQ, wg * 64, h, q0, b);
-        tma_store_commit();
+        tma_reduce_add_4d(&tmDQ, sDQ + kDQBox, wg * 64 + 32, h, q0, b);
+        tma_store_commit();  // one bulk group: the wait below covers both boxes
         if (turn) {
           tma_store_wait<0>();  // our reduction has been performed ...
           __threadfence();
@@ -494,8 +516,8 @@ extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_t
   if ((rc = make_tensor_map(&tmDO, d_o, B, Sq, H, D, dt, 2, 64, kBwdM, true))) return rc;
   if ((rc = make_tensor_map(&tmK, k, B, Sk, H_kv, D, dt, 2, 64, kBwdN, true))) return rc;
   if ((rc = make_tensor_map(&tmV, v, B, Sk, H_kv, D, dt, 2, 64, kBwdN, true))) return rc;
-  // dQ reductions: [64 rows][64 fp32 columns] boxes, no swizzle (one per reducing warpgroup), H query heads
-  if ((rc = make_tensor_map(&tmDQ, dq_acc, B, Sq, H, D, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 64, kBwdM, false)))
+  // dQ reductions: [64 rows][32 fp32 columns] SW128 boxes (two per reducing warpgroup), H query heads
+  if ((rc = make_tensor_map(&tmDQ, dq_acc, B, Sq, H, D, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 32, kBwdM, true)))
     return rc;
 
   BwdParams p;
