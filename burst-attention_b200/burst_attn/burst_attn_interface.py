@@ -210,6 +210,162 @@ def _bwd_rows(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causa
                   deterministic, **bkw)
 
 
+# --------------------------------------------------------------------------- #
+# sliding-window (local) attention: band masks per round
+# --------------------------------------------------------------------------- #
+def _check_window(window_size, causal):
+    """flash-attn's ``window_size=(left, right)`` (-1: that side unlimited; ``causal`` forces right = 0) ->
+    ``(left, right)`` with None for an unlimited side, or None when nothing is windowed: such a call runs exactly as
+    one without the argument."""
+    if window_size is None:
+        return None
+    try:
+        left, right = (int(x) for x in window_size)
+    except (TypeError, ValueError):
+        raise ValueError(f"window_size must be a pair (left, right) of ints, got {window_size!r}") from None
+    for name, x in (("left", left), ("right", right)):
+        if x < -1:
+            raise ValueError(f"window_size: {name} = {x}; it must be -1 (unlimited) or >= 0")
+    left = None if left == -1 else left
+    right = 0 if causal else (None if right == -1 else right)
+    if left is None and (right is None or causal):
+        return None
+    return left, right
+
+
+def _band(qn, kn, lo, hi):
+    """The band of a view of ``qn`` rows and ``kn`` keys -- key c visible to row a iff a + lo <= c <= a + hi (None:
+    that side open) -- with the sides that mask nothing opened, or None when no row sees any key (no launch)."""
+    if hi is not None and (qn - 1 + hi < 0 or (lo is not None and lo > hi)):
+        return None
+    if lo is not None and lo >= kn:
+        return None
+    if hi is not None and hi >= kn - 1:
+        hi = None
+    if lo is not None and lo <= 1 - qn:
+        lo = None
+    return lo, hi
+
+
+def _round_pieces(layout, W, iq, jk, S, window):
+    """The pieces of the round that attends the Q shard of rank ``iq`` to the K/V shard of rank ``jk`` (``S`` rows
+    each): ``[(q0, qn, k0, kn, lo, hi)]``, rows and keys local to the shards, the band relative to the two views;
+    pieces whose band misses its view are left out.  ``window`` = (left, right) counts positions in the full
+    sequence: contiguous shards start at rank * S, zigzag shards are the halves rank and 2W-1-rank (one piece per
+    pair of halves), and striped token a of rank r sits at a W + r, so a + ceil((iq-jk-left)/W) <= c <=
+    a + floor((iq-jk+right)/W)."""
+    left, right = window
+    if layout == "striped":
+        cand = [(0, S, 0, S, None if left is None else -((jk - iq + left) // W),
+                 None if right is None else (iq - jk + right) // W)]
+    else:
+        if layout == "contiguous":
+            qs, ks = [(0, S, iq * S)], [(0, S, jk * S)]
+        else:
+            assert S % 2 == 0, "zigzag causal sharding needs an even local sequence length"
+            h = S // 2
+            qs = [(0, h, iq * h), (h, h, (2 * W - 1 - iq) * h)]
+            ks = [(0, h, jk * h), (h, h, (2 * W - 1 - jk) * h)]
+        cand = [(qa, qn, ka, kn, None if left is None else qg - kg - left, None if right is None else qg - kg + right)
+                for qa, qn, qg in qs for ka, kn, kg in ks]
+    out = []
+    for qa, qn, ka, kn, lo, hi in cand:
+        b = _band(qn, kn, lo, hi)
+        if b is not None:
+            out.append((qa, qn, ka, kn) + b)
+    return out
+
+
+def _fwd_band_launches(pieces):
+    """Forward launches ``[(q0, qn, k0, kn, lo, hi)]`` of a round's pieces: a piece longer than the L2 block is split
+    over blocks of keys as in ``_fwd_blocks``, each launch taking only the rows that see its block."""
+    blk = _l2_block()
+    out = []
+    for qa, qn, ka, kn, lo, hi in pieces:
+        if kn <= blk + blk // 2:
+            out.append((qa, qn, ka, kn, lo, hi))
+            continue
+        for c0 in range(0, kn, blk):
+            cn = min(blk, kn - c0)
+            r0 = 0 if hi is None else max(0, c0 - hi)
+            r1 = qn if lo is None else min(qn, c0 + cn - lo)
+            b = _band(r1 - r0, cn, None if lo is None else lo + r0 - c0, None if hi is None else hi + r0 - c0) \
+                if r0 < r1 else None
+            if b is not None:
+                out.append((qa + r0, r1 - r0, ka + c0, cn) + b)
+    return out
+
+
+def _bwd_band_launches(pieces):
+    """Backward launches of a round's pieces: a piece with more rows than the L2 block is split over blocks of rows
+    as in ``_bwd_rows``, each launch taking only the keys its rows see."""
+    blk = _l2_block()
+    out = []
+    for qa, qn, ka, kn, lo, hi in pieces:
+        if qn <= blk + blk // 2:
+            out.append((qa, qn, ka, kn, lo, hi))
+            continue
+        for r0 in range(0, qn, blk):
+            rn = min(blk, qn - r0)
+            c0 = 0 if lo is None else max(0, r0 + lo)
+            c1 = kn if hi is None else min(kn, r0 + rn + hi)
+            b = _band(rn, c1 - c0, None if lo is None else lo + r0 - c0, None if hi is None else hi + r0 - c0) \
+                if c0 < c1 else None
+            if b is not None:
+                out.append((qa + r0, rn, ka + c0, c1 - c0) + b)
+    return out
+
+
+def _lower_kw(lo):
+    """Keyword for the chunk operators: the band's lower edge (nothing without one)."""
+    return {} if lo is None else {"lower": lo}
+
+
+class _BandForward:
+    """The launches of a windowed forward, known up front for every round, and their first / last duties.  Skipped
+    launches must not drop either: the state is started by the first launch only if it covers every row (otherwise
+    it starts as O = 0, lse = -inf in memory), and the output is written by the last launch only if it covers every
+    row (otherwise it is cast from the fp32 state at the end)."""
+
+    def __init__(self, rounds, q, lse, S):
+        flat = [x for launches in rounds for x in launches]
+        full = lambda x: x[0] == 0 and x[1] == S  # noqa: E731
+        self.first = bool(flat) and full(flat[0])
+        self.last = bool(flat) and full(flat[-1])
+        self.n, self.done = len(flat), 0
+        self.o_acc = None
+        if not (self.n == 1 and self.first and self.last):
+            self.o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device)
+        if not self.first:
+            self.o_acc.zero_()
+            lse.fill_(float("-inf"))
+
+    def run(self, ops, launches, q, k, v, lse, out, scale, seq_dim, bias=None):
+        for q0, qn, k0, kn, lo, hi in launches:
+            first = self.first and self.done == 0
+            last = self.last and self.done == self.n - 1
+            rows = lambda t: t.narrow(seq_dim, q0, qn)  # noqa: E731
+            ops.fwd_chunk(rows(q), k.narrow(seq_dim, k0, kn), v.narrow(seq_dim, k0, kn),
+                          None if self.o_acc is None else rows(self.o_acc), lse.narrow(2, q0, qn),
+                          rows(out) if last else None, scale, hi is not None, 0 if hi is None else hi, first, last,
+                          seq_dim, **_bias_kw(bias, k0, kn), **_lower_kw(lo))
+            self.done += 1
+
+    def finish(self, ops, out, seq_dim):
+        if not self.last:
+            ops.cast(self.o_acc, out, seq_dim)
+
+
+def _bwd_band_run(ops, launches, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic,
+                  bias=None):
+    for q0, qn, k0, kn, lo, hi in launches:
+        rows = lambda t: t.narrow(seq_dim, q0, qn)  # noqa: E731
+        keys = lambda t: t.narrow(seq_dim, k0, kn)  # noqa: E731
+        ops.bwd_chunk(rows(g), rows(q), keys(k), keys(v), delta.narrow(2, q0, qn), lse.narrow(2, q0, qn),
+                      rows(dq_part), keys(dk_acc), keys(dv_acc), scale, hi is not None, 0 if hi is None else hi, seq_dim,
+                      deterministic, **_bias_kw(bias, k0, kn), **_lower_kw(lo))
+
+
 def _check_inputs(q, k, v, seq_dim):
     assert q.dim() == 4 and k.shape == v.shape and q.shape[0] == k.shape[0] and q.shape[3] == k.shape[3], \
         "q, k, v must be 4-D with matching batch and head_dim"
@@ -245,8 +401,9 @@ def _fwd_dispatch(ops, mode, r, W, i, j, q, cur_k, cur_v, o_acc, lse, out, scale
 # --------------------------------------------------------------------------- #
 # forward ring (reference OpBurstAttn.forward :171-253, OpBurstAttnStrip.forward :411-493)
 # --------------------------------------------------------------------------- #
-def _ring_forward(q, k, v, scale, seq_dim, mode, topo):
-    """mode: "none" (non-causal) | "zigzag" | "striped".  Returns (out, lse[B,H,S] fp32).
+def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None):
+    """mode: "none" (non-causal) | "zigzag" | "striped".  Returns (out, lse[B,H,S] fp32).  With a ``window``
+    (``_check_window``) the rounds run the band launches of ``_round_pieces`` for the shard ``layout`` instead.
 
     Rounds run in M cycles of L steps (the flat ring is one cycle, L = W).  Within a cycle K/V hop round the
     intra-node ring; on the hierarchical ring (reference comm.py:187-254, SURVEY.md Appendix C) the block a
@@ -262,8 +419,14 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo):
         assert S % 2 == 0, "zigzag causal sharding needs an even local sequence length"
     out = torch.empty_like(q)
     lse = torch.empty((B, H, S), dtype=torch.float32, device=q.device)
-    need_state = W > 1 or _fwd_round_needs_state(k, seq_dim)
-    o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device) if need_state else None
+    band = None
+    if window is not None:
+        band = _BandForward([_fwd_band_launches(_round_pieces(layout, W, i, topo.source(r), S, window))
+                             for r in range(1, W + 1)], q, lse, S)
+        o_acc = None
+    else:
+        need_state = W > 1 or _fwd_round_needs_state(k, seq_dim)
+        o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device) if need_state else None
     if W > 1:
         k, v = k.contiguous(), v.contiguous()
     ring.begin(q, [_nbytes(k), _nbytes(v)] * min(2, L - 1))
@@ -279,13 +442,19 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo):
             if t != L - 1:
                 nxt = recv[(r - 1) % len(recv)]
                 ring.post(cur, nxt)
-            _fwd_dispatch(ops, mode, r, W, i, j, q, cur[0], cur[1], o_acc, lse, out, scale, seq_dim)
+            if band is None:
+                _fwd_dispatch(ops, mode, r, W, i, j, q, cur[0], cur[1], o_acc, lse, out, scale, seq_dim)
+            else:  # a round whose shard lies outside every row's window launches nothing
+                band.run(ops, _fwd_band_launches(_round_pieces(layout, W, i, j, S, window)), q, cur[0], cur[1], lse,
+                         out, scale, seq_dim)
             if t != L - 1:
                 ring.wait()
                 cur = nxt
             elif c != M - 1:
                 inter.wait()
                 cur = xbuf[c % len(xbuf)]
+    if band is not None:
+        band.finish(ops, out, seq_dim)
     return out, lse
 
 
@@ -315,7 +484,7 @@ def _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, sca
         raise ValueError(mode)
 
 
-def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, deterministic):
+def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, deterministic, window=None, layout=None):
     ops = get_ops()
     W, i = topo.W, topo.rank
     dev = q.device
@@ -332,7 +501,12 @@ def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, determini
     dv_acc = torch.zeros(v.shape, **f32)
 
     def round_kernel(r, j, bundle, dq_part):
-        _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, scale, seq_dim, deterministic)
+        if window is None:
+            _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, scale, seq_dim, deterministic)
+            return
+        dlt, g, qq, ls = bundle  # the bundle of rank j against the K/V at home: rows of j, keys of i
+        _bwd_band_run(ops, _bwd_band_launches(_round_pieces(layout, W, j, i, S, window)), g, qq, k, v, dlt, ls,
+                      dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic)
 
     bundle = [delta, d_o, q, lse.contiguous()]
     if W == 1:
@@ -446,8 +620,9 @@ def _bwd_rounds(ops, topo, round_kernel, bundle, q, seq_dim):
 
 # --------------------------------------------------------------------------- #
 def _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-             double_group):
+             double_group, window_size=(-1, -1)):
     assert not causal or flash == "cuda", "Causal attention only supported for Flash v2"
+    ctx.window = _check_window(window_size, causal)
     ctx.softmax_scale = 1 / math.sqrt(q.shape[-1]) if softmax_scale is None else softmax_scale
     ctx.flash = None if flash not in ["cuda", "triton"] else flash
     ctx.seq_dim = 1 if ctx.flash else 2
@@ -479,9 +654,14 @@ def _unpad(t, D):
     return t if t.shape[-1] == D else t[..., :D].contiguous()
 
 
-def _op_forward(ctx, q, k, v, mode):
+def _op_forward(ctx, q, k, v, mode, layout):
+    """mode: the schedule of the call without a window; layout: its shards ("contiguous" | "zigzag" | "striped"),
+    which a window needs even where the mask-free schedule does not."""
     ctx.host = False
     if q.device.type == "cpu" and getattr(get_ops(), "name", "") == "sm90":  # (tests inject CPU chunk operators)
+        if ctx.window is not None:
+            raise NotImplementedError("window_size is not supported with host-resident (pinned CPU) operands; pass "
+                                      "CUDA tensors")
         # host-resident operands (pinned CPU tensors, one rank): copies stream under the kernels (host_stream.py)
         from . import host_stream
         if not host_stream.is_host_call(q, k, v):
@@ -494,8 +674,8 @@ def _op_forward(ctx, q, k, v, mode):
         ctx.save_for_backward(*saved)
         return o_host
     (qp, kp, vp), ctx.head_dim = _pad_head_dim(get_ops(), [q, k, v])
-    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, mode, ctx.topo)
-    ctx.mode = mode
+    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, mode, ctx.topo, ctx.window, layout)
+    ctx.mode, ctx.layout = mode, layout
     ctx.save_for_backward(qp, kp, vp, lse, out)
     return _unpad(out, ctx.head_dim)
 
@@ -505,12 +685,12 @@ def _op_backward(ctx, grad_output):
         from . import host_stream
         grads = host_stream.backward(grad_output, ctx.saved_tensors, ctx.softmax_scale, ctx.seq_dim,
                                      ctx.mode != "none", _l2_block(), ctx.deterministic)
-        return tuple(grads) + (None,) * 7
+        return tuple(grads) + (None,) * 8
     q, k, v, lse, out = ctx.saved_tensors
     (g,), _ = _pad_head_dim(get_ops(), [grad_output])
     dq, dk, dv = _ring_backward(g, q, k, v, out, lse, ctx.softmax_scale, ctx.seq_dim, ctx.mode, ctx.topo,
-                                ctx.deterministic)
-    return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 7
+                                ctx.deterministic, ctx.window, ctx.layout)
+    return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 8
 
 
 class OpBurstAttn(torch.autograd.Function):
@@ -518,15 +698,16 @@ class OpBurstAttn(torch.autograd.Function):
     for Normal Attention (flash=None):  q, k, v: [B, N, S, H]
     for Flash ("cuda"/"triton"):        q, k, v: [B, S, N, H]
     Each rank passes its own sequence shard: contiguous when non-causal, zigzag
-    halves {i, 2W-1-i} when causal.
+    halves {i, 2W-1-i} when causal.  window_size: flash-attn's (left, right) sliding window over positions of
+    the full sequence (-1: unlimited side; causal forces right = 0).
     """
 
     @staticmethod
     def forward(ctx, q, k, v, softmax_scale=None, flash="cuda", causal=False, optimize_bwd_comm=False,
-                deterministic=False, process_group=None, double_group=[None, None]):
+                deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1)):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-                 double_group)
-        return _op_forward(ctx, q, k, v, "zigzag" if causal else "none")
+                 double_group, window_size)
+        return _op_forward(ctx, q, k, v, "zigzag" if causal else "none", "zigzag" if causal else "contiguous")
 
     @staticmethod
     def backward(ctx, grad_output):
@@ -534,14 +715,15 @@ class OpBurstAttn(torch.autograd.Function):
 
 
 class OpBurstAttnStrip(torch.autograd.Function):
-    """Striped-causal variant: rank i owns tokens {i, i+W, i+2W, ...}."""
+    """Striped-causal variant: rank i owns tokens {i, i+W, i+2W, ...} (with or without causal; a window then
+    counts positions of the full sequence as in OpBurstAttn)."""
 
     @staticmethod
     def forward(ctx, q, k, v, softmax_scale=None, flash="cuda", causal=False, optimize_bwd_comm=False,
-                deterministic=False, process_group=None, double_group=[None, None]):
+                deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1)):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-                 double_group)
-        return _op_forward(ctx, q, k, v, "striped" if causal else "none")
+                 double_group, window_size)
+        return _op_forward(ctx, q, k, v, "striped" if causal else "none", "striped")
 
     @staticmethod
     def backward(ctx, grad_output):
@@ -550,13 +732,15 @@ class OpBurstAttnStrip(torch.autograd.Function):
 
 def burst_attn_func_striped(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: float = None,
                             flash: str = "cuda", causal: bool = False, optimize_bwd_comm: bool = False,
-                            deterministic: bool = False, process_group=None, double_group=[None, None]):
+                            deterministic: bool = False, process_group=None, double_group=[None, None],
+                            window_size=(-1, -1)):
     return OpBurstAttnStrip.apply(q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic,
-                                  process_group, double_group)
+                                  process_group, double_group, window_size)
 
 
 def burst_attn_func(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: float = None,
                     flash: str = "cuda", causal: bool = False, optimize_bwd_comm: bool = False,
-                    deterministic: bool = False, process_group=None, double_group=[None, None]):
+                    deterministic: bool = False, process_group=None, double_group=[None, None],
+                    window_size=(-1, -1)):
     return OpBurstAttn.apply(q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic,
-                             process_group, double_group)
+                             process_group, double_group, window_size)

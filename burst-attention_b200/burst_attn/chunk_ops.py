@@ -69,18 +69,23 @@ class NativeOps:
         return {k: (len(v), sum(a.elapsed_time(b) for a, b in v)) for k, v in (self.timing or {}).items()}
 
     # ---- forward round: fold chunk (k, v) into (o_acc, lse); on last write o_out
-    def fwd_chunk(self, q, k, v, o_acc, lse, o_out, scale, causal, causal_offset, first, last, seq_dim, bias=None):
+    def fwd_chunk(self, q, k, v, o_acc, lse, o_out, scale, causal, causal_offset, first, last, seq_dim, bias=None,
+                  lower=None):
         """bias: optional fp32 [B|1, H, Sk] additive bias per key (expanded views with stride 0 over the batch are fine),
-        indexed by the query head."""
+        indexed by the query head.  lower: optional lower edge of a band mask, key c visible to row a only if
+        c >= a + lower (None: no lower edge)."""
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         flags = (_n.BA_FWD_FIRST if first else 0) | (_n.BA_FWD_LAST if last else 0)
         e0 = self._t0(q.device)
-        rc = self.lib.ba_fwd_chunk_gqa(
-            _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(bias), _n.t4(o_acc, seq_dim), _n.rs(lse),
-            _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale),
-            _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset), flags,
-            _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        args = (_n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(bias), _n.t4(o_acc, seq_dim), _n.rs(lse),
+                _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale),
+                _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
+        if lower is None:
+            rc = self.lib.ba_fwd_chunk_gqa(*args, flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        else:
+            args = args[:-2] + (args[-2] | _n.BA_MASK_LOWER, args[-1], int(lower))
+            rc = self.lib.ba_fwd_chunk_band(*args, flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
         _n.check(rc, "ba_fwd_chunk")
         self._shape("fwd_chunk_kernel", Sq, Sk, H, causal)
         self._t1("fwd_chunk_kernel", e0, q.device)
@@ -98,16 +103,20 @@ class NativeOps:
 
     # ---- backward round: accumulate into fp32 dq_acc / dk_acc / dv_acc
     def bwd_chunk(self, d_o, q, k, v, delta, lse, dq_acc, dk_acc, dv_acc, scale, causal, causal_offset, seq_dim,
-                  deterministic=False, bias=None):
+                  deterministic=False, bias=None, lower=None):
+        """lower: as in fwd_chunk."""
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         e0 = self._t0(q.device)
-        rc = self.lib.ba_bwd_chunk_gqa(
-            _n.t4(d_o, seq_dim), _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(delta), _n.rs(lse),
-            _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv, D,
-            float(scale),
-            _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset), 1 if deterministic else 0,
-            _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        args = (_n.t4(d_o, seq_dim), _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(delta), _n.rs(lse),
+                _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv,
+                D, float(scale), _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
+        tail = (1 if deterministic else 0, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        if lower is None:
+            rc = self.lib.ba_bwd_chunk_gqa(*args, *tail)
+        else:
+            args = args[:-2] + (args[-2] | _n.BA_MASK_LOWER, args[-1], int(lower))
+            rc = self.lib.ba_bwd_chunk_band(*args, *tail)
         _n.check(rc, "ba_bwd_chunk")
         self._shape("bwd_chunk_kernel", Sq, Sk, H, causal)
         self._t1("bwd_chunk_kernel", e0, q.device)

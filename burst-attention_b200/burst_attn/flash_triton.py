@@ -17,6 +17,11 @@ Grouped-query / multi-query attention as in flash-attn: ``flash_attn_func`` and 
 K/V with ``nheads_k`` heads where ``nheads_k`` divides ``nheads``; query head ``h`` attends with K/V head
 ``h // (nheads // nheads_k)``, and dK / dV come back with ``nheads_k`` heads (summed over each group).  A per-key bias
 is still ``(batch | 1, nheads, 1, seqlen_k)``, one row per query head.
+
+Sliding-window (local) attention as in flash-attn: ``window_size=(left, right)``, -1 for an unlimited side; query row
+``i`` sees key ``j`` iff ``i + Sk - Sq - left <= j <= i + Sk - Sq + right`` (the bottom-right alignment of ``causal``,
+which forces ``right = 0``).  The tile kernels skip the key tiles outside each row block's band.  A row that sees no
+key returns 0 and gets no gradient.
 """
 from __future__ import annotations
 
@@ -24,7 +29,9 @@ import math
 
 import torch
 
-from .burst_attn_interface import _bwd_round, _fwd_round, _fwd_round_needs_state, _pad_head_dim, _unpad
+from .burst_attn_interface import (_band, _BandForward, _bwd_band_launches, _bwd_band_run, _bwd_round,
+                                   _check_window, _fwd_band_launches, _fwd_round, _fwd_round_needs_state,
+                                   _pad_head_dim, _unpad)
 from .chunk_ops import get_ops
 
 __all__ = ["flash_attn_func", "flash_attn_kvpacked_func", "flash_attn_qkvpacked_func"]
@@ -42,19 +49,33 @@ def _key_bias(bias, q, k):
     return b3.expand(B, H, Sk)
 
 
-def _local_forward(q, k, v, causal, softmax_scale, bias=None):
+def _window_pieces(window, Sq, Sk):
+    """The one piece (``_round_pieces`` form) of a windowed local call, or none when no row sees a key."""
+    left, right = window
+    off = Sk - Sq
+    b = _band(Sq, Sk, None if left is None else off - left, None if right is None else off + right)
+    return [] if b is None else [(0, Sq, 0, Sk) + b]
+
+
+def _local_forward(q, k, v, causal, softmax_scale, bias=None, window=None):
     ops = get_ops()
     scale = softmax_scale or 1.0 / math.sqrt(q.shape[-1])
     (qp, kp, vp), D = _pad_head_dim(ops, [q, k, v])
     B, Sq, H = qp.shape[0], qp.shape[1], qp.shape[2]
     out = torch.empty(qp.shape, dtype=qp.dtype, device=qp.device)
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=qp.device)
+    if window is not None:
+        launches = _fwd_band_launches(_window_pieces(window, Sq, kp.shape[1]))
+        band = _BandForward([launches], qp, lse, Sq)
+        band.run(ops, launches, qp, kp, vp, lse, out, scale, 1, bias)
+        band.finish(ops, out, 1)
+        return out, lse, scale, (qp, kp, vp), D
     o_acc = torch.empty(qp.shape, dtype=torch.float32, device=qp.device) if _fwd_round_needs_state(kp, 1) else None
     _fwd_round(ops, qp, kp, vp, o_acc, lse, out, scale, causal, kp.shape[1] - Sq, True, True, 1, bias)
     return out, lse, scale, (qp, kp, vp), D
 
 
-def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, deterministic=False):
+def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, deterministic=False, window=None):
     ops = get_ops()
     (g,), _ = _pad_head_dim(ops, [do])
     g, out = g.contiguous(), out.contiguous()
@@ -63,6 +84,10 @@ def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, determin
     ops.delta(out, g, delta, 1)
     f32 = dict(dtype=torch.float32, device=qp.device)
     dq, dk, dv = torch.zeros(qp.shape, **f32), torch.zeros(kp.shape, **f32), torch.zeros(vp.shape, **f32)
+    if window is not None:
+        _bwd_band_run(ops, _bwd_band_launches(_window_pieces(window, Sq, kp.shape[1])), g, qp, kp, vp, delta, lse, dq,
+                      dk, dv, scale, 1, deterministic, bias)
+        return dq, dk, dv
     _bwd_round(ops, g, qp, kp, vp, delta, lse, dq, dk, dv, scale, causal, kp.shape[1] - Sq, 1, deterministic, bias)
     return dq, dk, dv
 
@@ -88,11 +113,13 @@ class FlashAttnFunc(torch.autograd.Function):
     (reference :1122-1168)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, bias=None, causal=False, softmax_scale=None):
+    def forward(ctx, q, k, v, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1)):
         _check(bias, q, k, v)
         _check_heads(q, k)
         ctx.bias = _key_bias(bias, q, k)
-        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, k, v, causal, softmax_scale, ctx.bias)
+        ctx.window = _check_window(window_size, causal)
+        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, k, v, causal, softmax_scale, ctx.bias,
+                                                                          ctx.window)
         ctx.save_for_backward(*saved, out, lse)
         ctx.causal = causal
         return _unpad(out, ctx.head_dim)
@@ -100,8 +127,10 @@ class FlashAttnFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
-        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias)
-        return _cast(dq, qp, ctx.head_dim), _cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim), None, None, None
+        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
+                                     window=ctx.window)
+        return (_cast(dq, qp, ctx.head_dim), _cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim), None, None, None,
+                None)
 
 
 class FlashAttnKVPackedFunc(torch.autograd.Function):
@@ -109,12 +138,13 @@ class FlashAttnKVPackedFunc(torch.autograd.Function):
     (reference :1073-1119)."""
 
     @staticmethod
-    def forward(ctx, q, kv, bias=None, causal=False, softmax_scale=None):
+    def forward(ctx, q, kv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1)):
         _check(bias, q, kv)
         _check_heads(q, kv[:, :, 0])
         ctx.bias = _key_bias(bias, q, kv[:, :, 0])
+        ctx.window = _check_window(window_size, causal)
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, kv[:, :, 0], kv[:, :, 1], causal,
-                                                                          softmax_scale, ctx.bias)
+                                                                          softmax_scale, ctx.bias, ctx.window)
         ctx.save_for_backward(*saved, out, lse)
         ctx.causal = causal
         return _unpad(out, ctx.head_dim)
@@ -122,20 +152,22 @@ class FlashAttnKVPackedFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
-        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias)
+        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
+                                     window=ctx.window)
         dkv = torch.stack([_cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim)], dim=2)
-        return _cast(dq, qp, ctx.head_dim), dkv, None, None, None
+        return _cast(dq, qp, ctx.head_dim), dkv, None, None, None, None
 
 
 class FlashAttnQKVPackedFunc(torch.autograd.Function):
     """qkv: (batch, seqlen, 3, nheads, headdim)  (reference :1021-1070)."""
 
     @staticmethod
-    def forward(ctx, qkv, bias=None, causal=False, softmax_scale=None):
+    def forward(ctx, qkv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1)):
         _check(bias, qkv)
         ctx.bias = _key_bias(bias, qkv[:, :, 0], qkv[:, :, 1])
+        ctx.window = _check_window(window_size, causal)
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal,
-                                                                          softmax_scale, ctx.bias)
+                                                                          softmax_scale, ctx.bias, ctx.window)
         ctx.save_for_backward(*saved, out, lse)
         ctx.causal = causal
         return _unpad(out, ctx.head_dim)
@@ -143,9 +175,10 @@ class FlashAttnQKVPackedFunc(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
-        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias)
+        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
+                                     window=ctx.window)
         dqkv = torch.stack([_cast(t, qp, ctx.head_dim) for t in (dq, dk, dv)], dim=2)
-        return dqkv, None, None, None
+        return dqkv, None, None, None, None
 
 
 flash_attn_func = FlashAttnFunc.apply

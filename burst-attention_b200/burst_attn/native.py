@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("BA_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "lib", "libburst_attn_b200.so")
 
 BA_DTYPE_FP16, BA_DTYPE_BF16 = 0, 1
-BA_MASK_NONE, BA_MASK_CAUSAL = 0, 1
+BA_MASK_NONE, BA_MASK_CAUSAL, BA_MASK_LOWER = 0, 1, 2
 BA_FWD_FIRST, BA_FWD_LAST = 1, 2
 NCCL_UNIQUE_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
@@ -49,12 +49,15 @@ _EXPORTS = {
     "ba_fwd_chunk": (_i, [_T4, _T4, _T4, _T4, _RS, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "ba_fwd_chunk_bias": (_i, [_T4, _T4, _T4, _RS, _T4, _RS, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "ba_fwd_chunk_gqa": (_i, [_T4, _T4, _T4, _RS, _T4, _RS, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_fwd_chunk_band": (_i, [_T4, _T4, _T4, _RS, _T4, _RS, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _i, _vp]),
     "ba_bwd_delta": (_i, [_T4, _T4, _RS, _i, _i, _i, _i, _i, _vp]),
     "ba_bwd_chunk": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _T4, _T4, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "ba_bwd_chunk_bias": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _RS, _T4, _T4, _T4,
                                _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "ba_bwd_chunk_gqa": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _RS, _T4, _T4, _T4,
                               _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
+    "ba_bwd_chunk_band": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _RS, _T4, _T4, _T4,
+                               _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _i, _vp]),
     "ba_cast_from_f32": (_i, [_T4, _T4, _i, _i, _i, _i, _i, _vp]),
     "ba_accumulate_f32": (_i, [_T4, _T4, _i, _i, _i, _i, _vp]),
     "ba_ring_unique_id": (_i, [_vp]),

@@ -1,353 +1,5 @@
-// ba_fwd_chunk: one ring round of the forward on sm_90a.
-//
-// Replaces, for flash="cuda"/"triton", the reference's per-round
-//   flash_attn_2_cuda.fwd  +  cuda_scale_out_lse_helper          (burst_utils.py:149-177, :20-33)
-// and the Triton LAO tile with carried state                       (lao.py:66-244)
-// by ONE kernel: the carried (O fp32 normalised, lse) state is loaded in the
-// prologue as the initial online-softmax state (m = lse, l = 1, acc = O) and the
-// merged state is written in the epilogue -- no separate merge pass over HBM.
-//
-// Grouped-query attention: K/V may have H / G heads; query head h reads K/V head h / G.  The grid is
-// (Q tiles, query heads, batch), so the G query heads of a group are adjacent in blockIdx.y and their CTAs sweep
-// the same K/V slice while it is resident in L2.
-//
-// Structure (one CTA = one 128-row Q tile of one (batch, head)):
-//   warpgroup 0   one TMA producer thread: Q once, then K_i / V_i tiles into 2-stage rings (and, with a key bias,
-//                 the tile's bias in log2 units); the other warps of the group only hand their registers over
-//   warpgroups 1, 2  64 Q rows each, everything in registers:
-//                 S = Q_w K_i^T      (wgmma SS m64n128, both operands K-major SW128 smem)
-//                 online softmax     (a thread owns 2 rows x 32 columns of S; row reductions over the quad)
-//                 O_w += P V_i       (wgmma RS: P re-packed to 16 bit in registers as the A operand, V MN-major)
-// The two consumer warpgroups run unsynchronised, so one group's softmax overlaps the other's MMAs.
-#include <math.h>
-#include <stdlib.h>
-
-#include "host_common.h"
-#include "sm90_ptx.cuh"
-
-namespace ba {
-
-constexpr int kBlockM = 128;  // Q rows per CTA (64 per consumer warpgroup)
-constexpr int kBlockN = 128;  // keys per K/V tile
-constexpr int kKStages = 2;
-constexpr int kVStages = 2;
-constexpr int kBoxBytes = 128 * 64 * 2;  // 16 KiB: one 128 x 64 SW128 TMA box (a [128][head_dim] tile is head_dim/64 boxes)
-constexpr int kFwdThreads = 384;         // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + softmax
-
-struct FwdParams {
-  float* o_acc;
-  int64_t oacc_sb, oacc_ss, oacc_sh;
-  float* lse;
-  int64_t lse_sb, lse_sh;
-  void* o_out;
-  int64_t oout_sb, oout_ss, oout_sh;
-  int B, Sq, Sk, H;
-  int G;              // query heads per K/V head (grouped-query attention; 1 = MHA): head h reads K/V head h / G
-  float scale_log2;
-  const float* bias;  // optional additive bias per key [B|1, H, Sk] (fp32, indexed by the query head), or null
-  int64_t bias_sb, bias_sh;
-  int causal;
-  int causal_off;
-  int load_state;
-  int store_lowp;
-};
-
-struct __align__(8) FwdBarriers {
-  uint64_t q_full;
-  uint64_t k_full[kKStages], k_empty[kKStages];
-  uint64_t b_full[kKStages];  // kBias: the key-bias row of this K stage has been written
-  uint64_t v_full[kVStages], v_empty[kVStages];
-};
-
-// shared-memory carve-up for head dim kD (64 or 128): a tile is [128 rows][kD] 16-bit = kD/64 SW128 boxes of
-// [128 rows][64 cols] (16 KiB each)
-template <int kD>
-struct FwdLayout {
-  static_assert(kD == 64 || kD == 128, "head dim 64 or 128");
-  static constexpr uint32_t kTileB = 128 * kD * 2;
-  static constexpr int kBoxes = kD / 64;
-  static constexpr uint32_t kOffQ = 0;
-  static constexpr uint32_t kOffK = kTileB;
-  static constexpr uint32_t kOffV = kOffK + kKStages * kTileB;
-  static constexpr uint32_t kOffBias = kOffV + kVStages * kTileB;  // [kKStages][128] fp32
-  static constexpr uint32_t kOffBars = kOffBias + kKStages * kBlockN * 4;
-  static constexpr int kSmemBytes = kOffBars + 256 /*barriers*/;
-  static_assert(kSmemBytes <= 232448, "forward kernel exceeds 227 KiB of shared memory");
-};
-
-// number of 128-key tiles the 64 Q rows starting at r0 must visit
-__device__ __forceinline__ int fwd_trip_count(int r0, const FwdParams& p) {
-  if (r0 >= p.Sq) return 0;
-  int r_last = min(r0 + 63, p.Sq - 1);
-  int max_limit = p.causal ? min(r_last + p.causal_off, p.Sk - 1) : p.Sk - 1;
-  return max_limit < 0 ? 0 : max_limit / kBlockN + 1;
-}
-
-template <bool kBF16, int kD, bool kBias>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((smem_u32(smem) & 1023u) != 0) __trap();      // SWIZZLE_128B atoms need a 1 KiB-aligned base
-  using L = FwdLayout<kD>;
-  constexpr uint32_t kTileBytes = L::kTileB;
-  constexpr int kBoxes = L::kBoxes, kOReg = kD / 2;  // fp32 accumulator registers of O per thread
-  uint8_t* sQ = smem + L::kOffQ;
-  uint8_t* sK = smem + L::kOffK;                    // [kKStages][tile]
-  uint8_t* sV = smem + L::kOffV;                    // [kVStages][tile]
-  float* sBias = reinterpret_cast<float*>(smem + L::kOffBias);
-  FwdBarriers* bars = reinterpret_cast<FwdBarriers*>(smem + L::kOffBars);
-
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
-  const int lane = threadIdx.x & 31;
-  const int h = blockIdx.y, b = blockIdx.z;
-  // causal: the last Q tiles see the most keys -- schedule them first (longest-processing-time order)
-  const int row0 = (p.causal ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x) * kBlockM;
-  const int n_tiles = max(fwd_trip_count(row0, p), fwd_trip_count(row0 + 64, p));
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    mbar_init(&bars->q_full, 1);
-    for (int i = 0; i < kKStages; ++i) {
-      mbar_init(&bars->k_full[i], 1);
-      mbar_init(&bars->k_empty[i], 8);  // one elected arrive per consumer warp
-      mbar_init(&bars->b_full[i], 1);
-    }
-    for (int i = 0; i < kVStages; ++i) {
-      mbar_init(&bars->v_full[i], 1);
-      mbar_init(&bars->v_empty[i], 8);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    // ============================================================ TMA producer (warp 0)
-    reg_alloc_dec<40>();
-    if (warp != 0) return;
-    const int hk = h / p.G;  // K/V head of this query head
-    if (lane == 0) {
-      mbar_arrive_expect_tx(&bars->q_full, kTileBytes);
-      for (int half = 0; half < kBoxes; ++half)
-        tma_load_4d(sQ + half * kBoxBytes, &tmQ, &bars->q_full, half * 64, h, row0, b);
-    }
-    for (int i = 0; i < n_tiles; ++i) {
-      const int ks = i % kKStages, kph = (i / kKStages) & 1;
-      mbar_wait(&bars->k_empty[ks], kph ^ 1);
-      if (lane == 0) {
-        mbar_arrive_expect_tx(&bars->k_full[ks], kTileBytes);
-        for (int half = 0; half < kBoxes; ++half)
-          tma_load_4d(sK + ks * kTileBytes + half * kBoxBytes, &tmK, &bars->k_full[ks], half * 64, hk,
-                      i * kBlockN, b);
-      }
-      if constexpr (kBias) {  // the stage's key bias in log2 units: lane handles keys lane + 32 j
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int key = i * kBlockN + lane + 32 * j;
-          float x = 0.f;
-          if (key < p.Sk) x = __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + key) * kLog2e;
-          sBias[ks * kBlockN + lane + 32 * j] = x;
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars->b_full[ks]);
-      }
-      if (lane == 0) {
-        const int vs = i % kVStages, vph = (i / kVStages) & 1;
-        mbar_wait(&bars->v_empty[vs], vph ^ 1);
-        mbar_arrive_expect_tx(&bars->v_full[vs], kTileBytes);
-        for (int half = 0; half < kBoxes; ++half)
-          tma_load_4d(sV + vs * kTileBytes + half * kBoxBytes, &tmV, &bars->v_full[vs], half * 64, hk,
-                      i * kBlockN, b);
-      }
-      __syncwarp();
-    }
-    return;
-  }
-
-  // ============================================================ consumers
-  reg_alloc_inc<232>();
-  const int wg = (threadIdx.x >> 7) - 1;  // 64-row half of the Q tile
-  const int w = warp & 3, g = lane >> 2, t = lane & 3;
-  const int r_lo = row0 + wg * 64 + 16 * w + g;  // this thread's two rows: r_lo and r_lo + 8
-  const int rows[2] = {r_lo, r_lo + 8};
-  const int n_mine = fwd_trip_count(row0 + wg * 64, p);
-  const float scale_log2 = p.scale_log2;
-  int limit[2];
-#pragma unroll
-  for (int r = 0; r < 2; ++r) limit[r] = p.causal ? min(rows[r] + p.causal_off, p.Sk - 1) : p.Sk - 1;
-  const int limit_min = min(limit[0], limit[1]);
-
-  float o[kOReg];
-  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // l: this thread's partial row sums
-#pragma unroll
-  for (int i = 0; i < kOReg; ++i) o[i] = 0.f;
-  if (p.load_state) {
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      if (rows[r] >= p.Sq) continue;
-      const float lse_prev = p.lse[(int64_t)b * p.lse_sb + (int64_t)h * p.lse_sh + rows[r]];
-      if (lse_prev != -INFINITY) {
-        m[r] = lse_prev * kLog2e;
-        l[r] = t == 0 ? 1.f : 0.f;  // counted once per row
-      }
-      const float* src = p.o_acc + (int64_t)b * p.oacc_sb + (int64_t)rows[r] * p.oacc_ss + (int64_t)h * p.oacc_sh;
-#pragma unroll
-      for (int c = 0; c < kD / 8; ++c) {
-        const float2 f = __ldg(reinterpret_cast<const float2*>(src + 8 * c + 2 * t));
-        o[4 * c + 2 * r] = f.x;
-        o[4 * c + 2 * r + 1] = f.y;
-      }
-    }
-  }
-
-  const uint32_t q_base = smem_u32(sQ) + wg * 64 * 128;  // this group's 64 rows inside every Q box
-  mbar_wait(&bars->q_full, 0);
-  for (int i = 0; i < n_tiles; ++i) {
-    const int ks = i % kKStages, kph = (i / kKStages) & 1;
-    const int vs = i % kVStages, vph = (i / kVStages) & 1;
-    const bool work = i < n_mine;  // warpgroup-uniform
-    mbar_wait(&bars->k_full[ks], kph);
-    float sc[64];
-    if (work) {
-      const uint32_t k_base = smem_u32(sK + ks * kTileBytes);
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < kD / 16; ++kk) {
-        const uint32_t off = (kk >> 2) * kBoxBytes + (kk & 3) * 32;
-        wgmma_ss_n128<kBF16, 0, 0>(sc, make_desc(q_base + off, 16, 1024), make_desc(k_base + off, 16, 1024),
-                                   kk > 0 ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs<64>(sc);
-      // scores in log2 units (+ key bias), masked keys -> -inf
-      const int key0 = i * kBlockN;
-      if constexpr (kBias) {
-        mbar_wait(&bars->b_full[ks], kph);
-        const float* bias = sBias + ks * kBlockN;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          const float2 bb = *reinterpret_cast<const float2*>(bias + 8 * c + 2 * t);
-#pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            sc[4 * c + 2 * r] = fmaf(sc[4 * c + 2 * r], scale_log2, bb.x);
-            sc[4 * c + 2 * r + 1] = fmaf(sc[4 * c + 2 * r + 1], scale_log2, bb.y);
-          }
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 64; ++j) sc[j] *= scale_log2;
-      }
-      if (key0 + kBlockN - 1 > limit_min) {
-#pragma unroll
-        for (int c = 0; c < 16; ++c)
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            if (key0 + 8 * c + 2 * t + (e & 1) > limit[e >> 1]) sc[4 * c + e] = -INFINITY;
-      }
-    }
-    // K (and the bias row) of this stage are no longer read by this warp
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars->k_empty[ks]);
-    if (work) {
-      uint32_t pa[32];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        float mx = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * r], sc[4 * c + 2 * r + 1]));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        const float m_new = fmaxf(m[r], mx);
-        const float f = (m[r] == -INFINITY) ? 0.f : ex2(m[r] - m_new);
-        const float neg_m = (m_new == -INFINITY) ? 0.f : -m_new;
-        m[r] = m_new;
-        float sum = 0.f;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          const float p0 = ex2(sc[4 * c + 2 * r] + neg_m), p1 = ex2(sc[4 * c + 2 * r + 1] + neg_m);
-          sc[4 * c + 2 * r] = p0;
-          sc[4 * c + 2 * r + 1] = p1;
-          sum += p0 + p1;
-        }
-        l[r] = l[r] * f + sum;
-#pragma unroll
-        for (int c = 0; c < kD / 8; ++c) {
-          o[4 * c + 2 * r] *= f;
-          o[4 * c + 2 * r + 1] *= f;
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < 32; ++j) pa[j] = pack2<kBF16>(sc[2 * j], sc[2 * j + 1]);
-      mbar_wait(&bars->v_full[vs], vph);
-      const uint32_t v_base = smem_u32(sV + vs * kTileBytes);
-      fence_regs<32>(pa);
-      fence_regs<kOReg>(o);
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < kBlockN / 16; ++kk) {
-        const uint64_t dv = make_desc(v_base + kk * 16 * 128, kBoxBytes, 1024);
-        if constexpr (kD == 128) wgmma_rs_n128<kBF16, 1>(o, pa + 4 * kk, dv, 1u);
-        else wgmma_rs_n64<kBF16, 1>(o, pa + 4 * kk, dv, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs<kOReg>(o);
-    } else {
-      mbar_wait(&bars->v_full[vs], vph);  // keeps the arrivals below in phase with the other warpgroup
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars->v_empty[vs]);
-  }
-
-  // ---------------------------------------------------------- epilogue
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    float lr = l[r];
-    lr += __shfl_xor_sync(0xffffffffu, lr, 1);
-    lr += __shfl_xor_sync(0xffffffffu, lr, 2);
-    const int row = rows[r];
-    if (row >= p.Sq) continue;
-    const float inv_l = lr > 0.f ? 1.f / lr : 0.f;
-    if (t == 0) p.lse[(int64_t)b * p.lse_sb + (int64_t)h * p.lse_sh + row] = lr > 0.f ? (m[r] + lg2(lr)) * kLn2 : -INFINITY;
-    if (p.store_lowp) {
-      uint16_t* dst = reinterpret_cast<uint16_t*>(p.o_out) + (int64_t)b * p.oout_sb + (int64_t)row * p.oout_ss +
-                      (int64_t)h * p.oout_sh + 2 * t;
-#pragma unroll
-      for (int c = 0; c < kD / 8; ++c)
-        *reinterpret_cast<uint32_t*>(dst + 8 * c) = pack2<kBF16>(o[4 * c + 2 * r] * inv_l, o[4 * c + 2 * r + 1] * inv_l);
-    } else {
-      float* dst = p.o_acc + (int64_t)b * p.oacc_sb + (int64_t)row * p.oacc_ss + (int64_t)h * p.oacc_sh + 2 * t;
-#pragma unroll
-      for (int c = 0; c < kD / 8; ++c)
-        *reinterpret_cast<float2*>(dst + 8 * c) = make_float2(o[4 * c + 2 * r] * inv_l, o[4 * c + 2 * r + 1] * inv_l);
-    }
-  }
-}
-
-
-static int launch_fwd(int dtype, int D, bool bias, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                      const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream) {
-  const bool bf16 = dtype == BA_DTYPE_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams);
-  if (bias)
-    kern = D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, true> : fwd_chunk_kernel<false, 64, true>)
-                   : (bf16 ? fwd_chunk_kernel<true, 128, true> : fwd_chunk_kernel<false, 128, true>);
-  else
-    kern = D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, false> : fwd_chunk_kernel<false, 64, false>)
-                   : (bf16 ? fwd_chunk_kernel<true, 128, false> : fwd_chunk_kernel<false, 128, false>);
-  const int smem = D == 64 ? FwdLayout<64>::kSmemBytes : FwdLayout<128>::kSmemBytes;
-  BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sq + kBlockM - 1) / kBlockM, p.H, p.B);
-  kern<<<grid, kFwdThreads, smem, stream>>>(tmQ, tmK, tmV, p);
-  BA_CHECK_CUDA(cudaGetLastError());
-  return BA_OK;
-}
-
-}  // namespace ba
+// ba_fwd_chunk*: the forward entry points, and the tile kernel without a band's lower edge (fwd_sm90.cuh).
+#include "fwd_sm90.cuh"
 
 extern "C" int ba_fwd_chunk(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse,
                             ba_tensor4 o_out, int B, int Sq, int Sk, int H, int D, float scale, int mask_mode,
@@ -367,9 +19,21 @@ extern "C" int ba_fwd_chunk_bias(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
 extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
                                 ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D,
                                 float scale, int mask_mode, int causal_offset, int flags, int dtype, void* stream) {
+  int rc;  // no band here: only BA_MASK_NONE / BA_MASK_CAUSAL
+  if ((rc = ba::check_chunk_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, mask_mode, dtype))) return rc;
+  return ba_fwd_chunk_band(q, k, v, key_bias, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode,
+                           causal_offset, 0, flags, dtype, stream);
+}
+
+extern "C" int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
+                                 ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D,
+                                 float scale, int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
+                                 void* stream) {
   using namespace ba;
   int rc;
-  if ((rc = check_chunk_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, mask_mode, dtype))) return rc;
+  if ((rc = check_band_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset, &lower_offset,
+                            dtype)))
+    return rc;
   BA_REQUIRE(q.ptr && k.ptr && v.ptr && lse.ptr, "ba_fwd_chunk: null q/k/v/lse");
   const bool first = flags & BA_FWD_FIRST, last = flags & BA_FWD_LAST;
   BA_REQUIRE(!last || o_out.ptr, "ba_fwd_chunk: BA_FWD_LAST needs o_out");
@@ -395,10 +59,14 @@ extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_row
   p.B = B, p.Sq = Sq, p.Sk = Sk, p.H = H;
   p.G = H / H_kv;
   p.scale_log2 = scale * kLog2e;
-  p.causal = mask_mode == BA_MASK_CAUSAL;
+  p.causal = (mask_mode & BA_MASK_CAUSAL) != 0;
   p.causal_off = causal_offset;
   p.load_state = first ? 0 : 1;
   p.store_lowp = last ? 1 : 0;
+  p.lo = lower_offset;
   p.bias = key_bias.ptr, p.bias_sb = key_bias.stride_b, p.bias_sh = key_bias.stride_h;
-  return launch_fwd(dtype, D, key_bias.ptr != nullptr, tmQ, tmK, tmV, p, static_cast<cudaStream_t>(stream));
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool bias = key_bias.ptr != nullptr;
+  if (mask_mode & BA_MASK_LOWER) return launch_fwd_band(dtype, D, bias, tmQ, tmK, tmV, p, st);
+  return launch_fwd<false>(dtype, D, bias, tmQ, tmK, tmV, p, st);
 }

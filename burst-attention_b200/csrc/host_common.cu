@@ -88,13 +88,32 @@ int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int
   return BA_OK;
 }
 
+int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
+                    int causal_offset, int* lower_offset, int dtype) {
+  const int mm = *mask_mode;
+  BA_REQUIRE((mm & ~(BA_MASK_CAUSAL | BA_MASK_LOWER)) == 0, "%s: bad mask mode %d", fn, mm);
+  int rc;
+  if ((rc = check_chunk_args(fn, B, Sq, Sk, H, H_kv, D, scale, mm & BA_MASK_CAUSAL, dtype))) return rc;
+  if (!(mm & BA_MASK_LOWER)) return BA_OK;
+  BA_REQUIRE(!(mm & BA_MASK_CAUSAL) || *lower_offset <= causal_offset,
+             "%s: band lower_offset %d is above its causal_offset %d (no key would be visible)", fn, *lower_offset,
+             causal_offset);
+  // a lower edge at or below key 0 for every row (lower_offset <= 1 - Sq) masks nothing: run the kernel without one;
+  // one at or above Sk masks every key of every row, as lower_offset = Sk does (and row + Sk cannot overflow)
+  if (*lower_offset <= 1 - Sq) *mask_mode = mm & ~BA_MASK_LOWER;
+  else if (*lower_offset > Sk) *lower_offset = Sk;
+  return BA_OK;
+}
+
 }  // namespace ba
 
 #ifdef BA_SELFTEST_LIB
 extern "C" const char* ba_selftest_last_error(void) { return ba::g_err; }
 #else
 extern "C" const char* ba_last_error(void) { return ba::g_err; }
-extern "C" int ba_version(void) { return 201; }  // 201: grouped-query attention (ba_fwd_chunk_gqa, ba_bwd_chunk_gqa)
+// 201: grouped-query attention (ba_fwd_chunk_gqa, ba_bwd_chunk_gqa); 202: band masks (ba_fwd_chunk_band,
+// ba_bwd_chunk_band)
+extern "C" int ba_version(void) { return 202; }
 extern "C" int ba_device_check(void) {
   int dev = 0;
   BA_CHECK_CUDA(cudaGetDevice(&dev));

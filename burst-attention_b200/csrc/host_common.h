@@ -53,4 +53,10 @@ inline bool aligned16(const ba_tensor4& t, int esize) {
 int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
                      int dtype);
 
+// The same for the band entry points, whose mask_mode is a set of BA_MASK_CAUSAL and BA_MASK_LOWER bits.  On
+// success it normalises the band: a lower edge that masks nothing is dropped from *mask_mode, and *lower_offset is
+// clamped to Sk.
+int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
+                    int causal_offset, int* lower_offset, int dtype);
+
 }  // namespace ba

@@ -39,6 +39,7 @@ extern "C" {
 /* mask modes (SURVEY.md Appendix B) */
 #define BA_MASK_NONE 0
 #define BA_MASK_CAUSAL 1 /* key j visible to query i iff j <= i + causal_offset */
+#define BA_MASK_LOWER 2  /* band entry points only: key j visible to query i only if j >= i + lower_offset */
 
 /* flags for ba_fwd_chunk */
 #define BA_FWD_FIRST 1 /* no carried state: start from (O=0, lse=-inf)                       */
@@ -96,6 +97,15 @@ int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bi
                      ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
                      int causal_offset, int flags, int dtype, void* stream);
 
+/* Band mask (sliding-window / local attention): the same as ba_fwd_chunk_gqa with mask_mode a set of bits,
+ * BA_MASK_CAUSAL (key j visible to query i only if j <= i + causal_offset) and BA_MASK_LOWER (only if
+ * j >= i + lower_offset); either side may be open.  With both bits lower_offset <= causal_offset is required.  A row
+ * that sees no key has lse = -inf and O = 0 (or keeps its carried state).  The CTA of a 128-row Q tile loads only the
+ * K/V tiles its band reaches.  ba_fwd_chunk_gqa is this call with BA_MASK_LOWER clear.                        */
+int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc, ba_rowstat lse,
+                      ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
+                      int causal_offset, int lower_offset, int flags, int dtype, void* stream);
+
 /* delta[b,h,s] = sum_d O[b,s,h,d] * dO[b,s,h,d]  (burst_attn_interface.py:272-278) */
 int ba_bwd_delta(ba_tensor4 o, ba_tensor4 d_o, ba_rowstat delta, int B, int S, int H, int D, int dtype,
                  void* stream);
@@ -121,6 +131,14 @@ int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, b
                      ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq, int Sk,
                      int H, int H_kv, int D, float scale, int mask_mode, int causal_offset, int flags, int dtype,
                      void* stream);
+
+/* Band mask: the same as ba_bwd_chunk_gqa with the mask bits and lower_offset of ba_fwd_chunk_band.  The CTA of a
+ * 128-key block visits only the 64-row Q blocks whose band reaches it; keys no row sees get dK = dV = 0 added.
+ * BA_BWD_DETERMINISTIC stays bitwise reproducible.  ba_bwd_chunk_gqa is this call with BA_MASK_LOWER clear.      */
+int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
+                      ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq,
+                      int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset, int lower_offset,
+                      int flags, int dtype, void* stream);
 
 /* dst[b,s,h,d] (dtype) = src[b,s,h,d] (fp32); used once per backward to hand the
  * fp32 gradient accumulators back in the input dtype.                              */
