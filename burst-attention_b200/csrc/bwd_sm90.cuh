@@ -10,24 +10,31 @@
 // One CTA owns one 128-key block of the home K/V chunk for one (batch, K/V head) and loops over the G query heads
 // that share that K/V head (grouped-query attention; G = 1 for MHA) and, for each, over the 64-row blocks of the
 // visiting Q-bundle: G x n_it steps, one pipeline whose stages and mbarrier phases run on across heads.
-// Warpgroup 0 is the TMA producer (K, V once; Q, dO and the row statistics per step, 2 stages); warpgroups 1 and 2
+// Warpgroup 0 is the TMA producer (K, V once; Q, dO and the row statistics per step, 3 stages); warpgroups 1 and 2
 // own 64 keys each and keep their dK, dV accumulators in registers across all G heads, so the epilogue does a
 // single read-modify-write of dk_acc / dv_acc per CTA (no atomics; dK / dV stay deterministic):
 //   S^T  = K_w Q_i^T,  dP^T = V_w dO_i^T      (wgmma SS m64n64, K-major operands)
 //   P^T  = exp2(S^T c [+ bias] - lse2),  dS^T = P^T o (dP^T - delta)     (registers, thread = 2 key rows)
-//   dV_w += P^T dO_i,  dK_w += dS^T Q_i       (wgmma RS: P^T / dS^T re-packed to 16 bit as the A operand,
-//                                               dO / Q read MN-major)
-//   dS^T -> smem (double-buffered), then dQ_i = dS K  (wgmma SS, both operands MN-major; head dim 128: each
-//   warpgroup computes 64 of the dQ columns, head dim 64: warpgroup 1 alone) -> smem -> cp.reduce.async.bulk.tensor
-//   (fp32 add in L2) into dq_acc.
-// Per step a consumer warpgroup keeps its own MMAs running under its element-wise work (five commit groups; four,
-// without dQ, for the non-reducing warpgroup at head dim 64):
-//   issue S^T | issue dP^T | wait<1>: P^T (exp2, bias, masks) + pack, under dP^T | wait<0> | issue dV |
-//   dS^T + pack + store to smem, under dV | barrier with the other warpgroup | issue dQ | issue dK |
-//   wait<1> (dV, dQ done): stage dQ + reduce-add, under dK | wait<0> | release the Q / dO stage.
-// The packed A operands (P^T for dV, dS^T for dK) stay untouched until the wait that retires their group.
-// smem (D = 128): K 32K, V 32K, Q 2x16K, dO 2x16K, dS^T 2x16K, dQ staging 16K per reducing warpgroup (single-
-// buffered: its next write waits for the previous reduce to have read it), row statistics 1K.
+//   dS^T -> smem (double-buffered)
+//   dV_w += P^T dO_i   (wgmma RS: P^T re-packed to 16 bit as the A operand, dO read MN-major)
+//   dK_w += dS^T Q_i   (wgmma SS: the warpgroup's rows of the dS^T tile read K-major, Q read MN-major)
+//   dQ_i = dS K        (wgmma SS, both operands MN-major; head dim 128: each warpgroup computes 64 of the dQ
+//                       columns, head dim 64: warpgroup 1 alone) -> smem -> cp.reduce.async.bulk.tensor (fp32 add
+//                       in L2) into dq_acc.
+// A consumer warpgroup keeps its own MMAs running under its element-wise work, and across steps: the next step's
+// S^T is issued between this step's dQ and dK, so the tensor cores have S^T and dK queued under the dQ staging, and
+// dK and the next dP^T under the next P^T (five commit groups per step; four, without dQ, for the non-reducing
+// warpgroup at head dim 64):
+//   prologue: issue S^T_0 | empty group (stands for dK_{-1}) | issue dP^T_0
+//   step j:   wait<2> (S^T_j done) | P^T (exp2, bias, masks) + pack, under dK_{j-1} and dP^T_j | wait<0> | release
+//             the Q / dO stage of step j-1 | issue dV | dS^T + pack + store to smem, under dV | barrier with the
+//             other warpgroup | issue dQ | issue S^T_{j+1} | issue dK | wait<2> (dV, dQ done) | stage dQ +
+//             reduce-add, under S^T_{j+1} and dK | issue dP^T_{j+1}
+//   the last step issues nothing for a next one and ends with wait<0> and the release of its stage.
+// The operands of an MMA (packed P^T for dV, the dS^T tile for dQ and dK) stay untouched until the wait that retires
+// its group.
+// smem (D = 128): K 32K, V 32K, Q 3x16K, dO 3x16K, dS^T 2x16K, dQ staging 16K per reducing warpgroup (single-
+// buffered: its next write waits for the previous reduce to have read it), row statistics 1.5K.
 // The dQ staging of a warpgroup is two [64 rows][32 fp32] SW128 boxes, one reduce-add each; lanes with odd row
 // index store their 8-column chunks in a permuted order, so every STS.64 of the staging is conflict-free (2
 // wavefronts; the bank arithmetic is next to the stores).
@@ -39,6 +46,8 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "host_common.h"
 #include "sm90_ptx.cuh"
 
@@ -47,6 +56,9 @@ namespace ba {
 constexpr int kBwdThreads = 384;  // warpgroup 0: loader (warp 0); warpgroups 1, 2: MMA + element-wise
 constexpr int kBwdN = 128;        // keys per CTA
 constexpr int kBwdM = 64;         // query rows per block of the Q-bundle
+// Q / dO / statistics stages.  A stage is released at the top of the step after the one that read it, and the
+// next step's stage is needed in the middle of a step, so with 3 stages the loader has about 1.5 steps per load.
+constexpr int kBwdStages = 3;
 
 struct BwdParams {
   const float* lse;
@@ -79,9 +91,10 @@ __device__ __forceinline__ void st_release_gpu(int* p, int v) {
 
 struct __align__(8) BwdBarriers {
   uint64_t kv_full;
-  uint64_t q_full[2], q_empty[2];  // Q, dO and the row statistics of one Q block
-  int key_block;                   // deterministic mode: this CTA's ticket
+  uint64_t q_full[kBwdStages], q_empty[kBwdStages];  // Q, dO and the row statistics of one Q block
+  int key_block;                                     // deterministic mode: this CTA's ticket
 };
+static_assert(sizeof(BwdBarriers) <= 64, "BwdLayout reserves 64 bytes for the barriers");
 
 // smem carve-up (bytes from the 1 KiB-aligned base); head dim kD (64 or 128)
 template <int kD>
@@ -93,12 +106,12 @@ struct BwdLayout {
   static constexpr int kBoxDQ = kBwdM * 128;  // 8 KiB: [64 rows][32 fp32 cols] SW128 box
   static constexpr int kOffK = 0;
   static constexpr int kOffV = kOffK + kBoxes * kBoxKV;
-  static constexpr int kOffQ = kOffV + kBoxes * kBoxKV;     // 2 stages
-  static constexpr int kOffDO = kOffQ + 2 * kBoxes * kBoxQ;  // 2 stages
-  static constexpr int kOffDS = kOffDO + 2 * kBoxes * kBoxQ; // 2 x [128 keys][64 q] SW128
-  static constexpr int kOffDQ = kOffDS + 2 * kBwdN * 128;    // per reducing warpgroup 2 dQ boxes (64 columns)
-  static constexpr int kOffStat = kOffDQ + kBoxes * 2 * kBoxDQ;  // 2 stages x [lse2 | delta] x 64 fp32
-  static constexpr int kOffBar = kOffStat + 2 * 2 * kBwdM * 4;
+  static constexpr int kOffQ = kOffV + kBoxes * kBoxKV;                // kBwdStages stages
+  static constexpr int kOffDO = kOffQ + kBwdStages * kBoxes * kBoxQ;   // kBwdStages stages
+  static constexpr int kOffDS = kOffDO + kBwdStages * kBoxes * kBoxQ;  // 2 x [128 keys][64 q] SW128
+  static constexpr int kOffDQ = kOffDS + 2 * kBwdN * 128;              // per reducing warpgroup 2 dQ boxes (64 columns)
+  static constexpr int kOffStat = kOffDQ + kBoxes * 2 * kBoxDQ;  // kBwdStages stages x [lse2 | delta] x 64 fp32
+  static constexpr int kOffBar = kOffStat + kBwdStages * 2 * kBwdM * 4;
   static constexpr int kSmemBytes = kOffBar + 64;  // no align slack: the dynamic smem base is checked to be 1 KiB aligned
   static_assert(kSmemBytes <= 232448, "backward kernel exceeds 227 KiB of shared memory");
   static_assert(kOffDQ % 1024 == 0, "SW128 dQ staging boxes need 1 KiB alignment");
@@ -154,7 +167,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     tma_prefetch_desc(&tmDO);
     tma_prefetch_desc(&tmDQ);
     mbar_init(&bars->kv_full, 1);
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < kBwdStages; ++s) {
       mbar_init(&bars->q_full[s], 1);
       mbar_init(&bars->q_empty[s], 8);  // one elected arrive per consumer warp
     }
@@ -174,10 +187,10 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
     }
     int it = 0, h = h0;  // Q block (relative to i_begin) and query head of this step
+    int st = 0, ph = 0;  // stage of this step (step % kBwdStages) and its phase ((step / kBwdStages) & 1)
     for (int step = 0; step < n_steps; ++step) {
       const int q0 = (i_begin + it) * kBwdM;
-      const int st = step & 1;
-      mbar_wait(&bars->q_empty[st], ((step >> 1) & 1) ^ 1);
+      mbar_wait(&bars->q_empty[st], ph ^ 1);
       // row statistics of this Q block (lane handles rows lane, lane + 32): lse in log2 units, delta
       float* stat = sStat + st * 2 * kBwdM;
 #pragma unroll
@@ -202,6 +215,7 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
       __syncwarp();
       if (++it == n_it) it = 0, ++h;
+      if (++st == kBwdStages) st = 0, ph ^= 1;
     }
     return;
   }
@@ -218,224 +232,270 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   // "vector" bias): a per-row scalar in this key-row layout, folded into the exponent's FMA; the bias is per query
   // head, so it is (re)loaded at the first step of every head
   float bias2[2];
-  const bool reducer = kD == 128 || wg == 0;  // owns 64 columns of dQ
   const int n_red = kD == 128 ? 2 : 1;
 
   float dk[kAcc], dv[kAcc];
 #pragma unroll
   for (int i = 0; i < kAcc; ++i) dk[i] = dv[i] = 0.f;
+  // the zeros are set here, not sunk under the first MMAs (writing an accumulator register while a wgmma group is in
+  // flight makes ptxas serialize every wgmma of the kernel)
+  fence_regs<kAcc>(dk);
+  fence_regs<kAcc>(dv);
 
   const uint32_t sK = smem_u32(smem + L::kOffK), sV = smem_u32(smem + L::kOffV);
   const uint32_t kw = wg * 64 * 128;  // this group's 64 key rows inside every K / V box
   uint8_t* sDQ = smem + L::kOffDQ + wg * 2 * kDQBox;
-  mbar_wait(&bars->kv_full, 0);
-  int it = 0, h = h0;  // Q block (relative to i_begin) and query head of this step
-  for (int step = 0; step < n_steps; ++step) {
-    const int q0 = (i_begin + it) * kBwdM;
-    const int st = step & 1;
-    const uint32_t sQ = smem_u32(smem + L::kOffQ + st * kQStageB), sDO = smem_u32(smem + L::kOffDO + st * kQStageB);
-    const float* stat = sStat + st * 2 * kBwdM;
-    if (it == 0) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r)
-        bias2[r] = (p.bias && keys[r] < p.Sk)
-                       ? __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + keys[r]) * kLog2e
-                       : 0.f;
-    }
-    mbar_wait(&bars->q_full[st], (step >> 1) & 1);
-
-    // S^T and dP^T as two commit groups: P^T is computed from S^T while dP^T is still running
-    float s[32], dp[32];
+  auto q_stage = [&](int st) { return smem_u32(smem + L::kOffQ + st * kQStageB); };
+  auto do_stage = [&](int st) { return smem_u32(smem + L::kOffDO + st * kQStageB); };
+  // acc = X_w Y^T as one commit group (wgmma SS m64n64, K-major operands): S^T = K_w Q^T or dP^T = V_w dO^T
+  auto issue_xt = [&](float* acc, uint32_t sX, uint32_t sY) {
+    // the descriptors are rebuilt at each issue: hoisted out of the step loop, the K ones would hold 16 registers
+    // for the whole step, and the step would spill
+    asm volatile("" : "+r"(sX));
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kD / 16; ++kk) {
       const uint32_t okv = (kk >> 2) * kBoxKV + kw + (kk & 3) * 32, oq = (kk >> 2) * kBoxQ + (kk & 3) * 32;
-      wgmma_ss_n64<kBF16, 0, 0>(s, make_desc(sK + okv, 16, 1024), make_desc(sQ + oq, 16, 1024), kk > 0 ? 1u : 0u);
+      wgmma_ss_n64<kBF16, 0, 0>(acc, make_desc(sX + okv, 16, 1024), make_desc(sY + oq, 16, 1024), kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
-#pragma unroll
-    for (int kk = 0; kk < kD / 16; ++kk) {
-      const uint32_t okv = (kk >> 2) * kBoxKV + kw + (kk & 3) * 32, oq = (kk >> 2) * kBoxQ + (kk & 3) * 32;
-      wgmma_ss_n64<kBF16, 0, 0>(dp, make_desc(sV + okv, 16, 1024), make_desc(sDO + oq, 16, 1024), kk > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<1>();  // S^T done, dP^T may still run
-    fence_regs<32>(s);
+  };
+  mbar_wait(&bars->kv_full, 0);
 
-    // P^T in place of S^T (fp32, kept for dS^T) and packed to 16 bit as the A operand of dV.
-    // visible iff key <= q + off  <=>  q >= key - off ; whole block visible when q0 + off >= k0 + 127
-    const bool need_mask = p.causal && (q0 + p.causal_off < k0 + kBwdN - 1);
-    // band: visible only if key >= q + lo; the whole block passes when k0 >= q0 + 63 + lo
-    const bool need_lo = kBand && (q0 + kBwdM - 1 + p.lo > k0);
-    uint32_t pp[16], ds[16];
+  // The steps of one consumer warpgroup.  kRed: it owns 64 columns of dQ (both warpgroups at head dim 128,
+  // warpgroup 1 alone at head dim 64).  dK of a step is retired in the next one, so the role is fixed for the whole
+  // loop rather than branched on per step: each wgmma group is issued and waited for on one path (a group across a
+  // divergent path makes ptxas serialize every wgmma of the kernel).
+  auto consume = [&](auto red) {
+    constexpr bool kRed = decltype(red)::value;
+    float s[32], dp[32];  // S^T (P^T in place) and dP^T of this step: issued by the step before
+    int it = 0, h = h0;   // Q block (relative to i_begin) and query head of this step
+    int st = 0, ph = 0;   // Q / dO / statistics stage of this step and its q_full phase
+    mbar_wait(&bars->q_full[0], 0);
+    issue_xt(s, sK, q_stage(0));
+    wgmma_commit();  // an empty group in the place of the previous step's dK, so that every step waits alike
+    issue_xt(dp, sV, do_stage(0));
+
+    // One step; kNext (every step but the last): issue the next step's S^T and dP^T.  The last step is a copy of
+    // its own, so that no wgmma is issued under a runtime condition.
+    auto step_body = [&](auto next, int step) {
+      constexpr bool kNext = decltype(next)::value;
+      const int q0 = (i_begin + it) * kBwdM;
+      const uint32_t sQ = q_stage(st), sDO = do_stage(st);
+      const float* stat = sStat + st * 2 * kBwdM;
+      if (it == 0) {
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const float2 l2 = *reinterpret_cast<const float2*>(stat + 8 * c + 2 * t);
+        for (int r = 0; r < 2; ++r)
+          bias2[r] = (p.bias && keys[r] < p.Sk)
+                         ? __ldg(p.bias + (int64_t)b * p.bias_sb + (int64_t)h * p.bias_sh + keys[r]) * kLog2e
+                         : 0.f;
+      }
+      // in flight, oldest first: S^T, dK of the previous step, dP^T; P^T is computed from S^T while the other two run
+      wgmma_wait<2>();  // S^T done
+      fence_regs<32>(s);
+
+      // P^T in place of S^T (fp32, kept for dS^T) and packed to 16 bit as the A operand of dV.
+      // visible iff key <= q + off  <=>  q >= key - off ; whole block visible when q0 + off >= k0 + 127
+      const bool need_mask = p.causal && (q0 + p.causal_off < k0 + kBwdN - 1);
+      // band: visible only if key >= q + lo; the whole block passes when k0 >= q0 + 63 + lo
+      const bool need_lo = kBand && (q0 + kBwdM - 1 + p.lo > k0);
+      uint32_t pp[16];
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int e = 4 * c + 2 * r;
-        float p0 = ex2(fmaf(s[e], scale_log2, bias2[r] - l2.x));
-        float p1 = ex2(fmaf(s[e + 1], scale_log2, bias2[r] - l2.y));
-        if (keys[r] >= p.Sk) p0 = p1 = 0.f;
-        if (need_mask) {
-          const int q = q0 + 8 * c + 2 * t;
-          if (q < keys[r] - p.causal_off) p0 = 0.f;
-          if (q + 1 < keys[r] - p.causal_off) p1 = 0.f;
-        }
-        if constexpr (kBand) {
-          if (need_lo) {
+      for (int c = 0; c < 8; ++c) {
+        const float2 l2 = *reinterpret_cast<const float2*>(stat + 8 * c + 2 * t);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int e = 4 * c + 2 * r;
+          float p0 = ex2(fmaf(s[e], scale_log2, bias2[r] - l2.x));
+          float p1 = ex2(fmaf(s[e + 1], scale_log2, bias2[r] - l2.y));
+          if (keys[r] >= p.Sk) p0 = p1 = 0.f;
+          if (need_mask) {
+            const int q = q0 + 8 * c + 2 * t;
+            if (q < keys[r] - p.causal_off) p0 = 0.f;
+            if (q + 1 < keys[r] - p.causal_off) p1 = 0.f;
+          }
+          if (need_lo) {  // false at compile time without kBand
             const int q = q0 + 8 * c + 2 * t;
             if (q + p.lo > keys[r]) p0 = 0.f;
             if (q + 1 + p.lo > keys[r]) p1 = 0.f;
           }
+          s[e] = p0, s[e + 1] = p1;
+          pp[2 * c + r] = pack2<kBF16>(p0, p1);
         }
-        s[e] = p0, s[e + 1] = p1;
-        pp[2 * c + r] = pack2<kBF16>(p0, p1);
       }
-    }
 
-    // dV += P^T dO   (B operand: [q rows][d] tile read MN-major); pp is read by the MMA until the wait<1> below
-    wgmma_wait<0>();  // dP^T done
-    fence_regs<32>(dp);
-    fence_regs<16>(pp);
-    fence_regs<kAcc>(dv);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < kBwdM / 16; ++kk) {
-      const uint64_t d_do = make_desc(sDO + kk * 16 * 128, kBoxQ, 1024);
-      if constexpr (kD == 128) wgmma_rs_n128<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
-      else wgmma_rs_n64<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
-    }
-    wgmma_commit();
-
-    // dS^T = P^T o (dP^T - delta) while dV runs
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      const float2 dl = *reinterpret_cast<const float2*>(stat + kBwdM + 8 * c + 2 * t);
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int e = 4 * c + 2 * r;
-        ds[2 * c + r] = pack2<kBF16>(s[e] * (dp[e] - dl.x), s[e + 1] * (dp[e + 1] - dl.y));
+      // dV += P^T dO   (B operand: [q rows][d] tile read MN-major); pp is read by the MMA until the wait<1> below
+      wgmma_wait<0>();  // dK of the previous step and dP^T done
+      fence_regs<32>(dp);
+      fence_regs<16>(pp);
+      fence_regs<kAcc>(dv);
+      fence_regs<kAcc>(dk);
+      if (step > 0) {
+        // dK of the previous step was the last reader of that step's Q, dO and statistics
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->q_empty[st == 0 ? kBwdStages - 1 : st - 1]);
       }
-    }
-
-    // dS^T -> smem [128 keys][64 q] (SW128: 16-byte chunk j of row r at j ^ (r % 8)), double-buffered: the buffer
-    // written here was last read by the dQ MMAs of step - 2.  Each reducing warpgroup's wgmma_wait<1> of step - 2
-    // completes its dQ group (dV and dQ are the two oldest of its three groups), and that wait comes before the
-    // warpgroup reaches the barrier of step - 1, which this warpgroup has passed.
-    uint8_t* sDS = smem + L::kOffDS + st * kBwdN * 128;
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int kr = kr_lo + 8 * r;
-        *reinterpret_cast<uint32_t*>(sDS + kr * 128 + ((c ^ (kr & 7)) << 4) + 4 * t) = ds[2 * c + r];
-      }
-    fence_proxy_async_smem();
-    named_bar_sync(1, 256);
-
-    // dQ[:, 64 wg .. 64 wg + 63] = dS K  (A = dS^T tile read MN-major, B = K tile read MN-major), then
-    // dK += dS^T Q (B operand read MN-major) as the last group: it runs on under the dQ staging below
-    // (head dim 64: the non-reducing warpgroup issues dK alone; each role runs its whole issue-to-wait sequence in
-    // one branch, so that no wgmma group crosses a divergent path, which would make ptxas serialize them)
-    float dq[32];
-    fence_regs<16>(ds);
-    fence_regs<kAcc>(dk);
-    auto issue_dk = [&]() {
+      wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kBwdM / 16; ++kk) {
-        const uint64_t d_q = make_desc(sQ + kk * 16 * 128, kBoxQ, 1024);
-        if constexpr (kD == 128) wgmma_rs_n128<kBF16, 1>(dk, ds + 4 * kk, d_q, 1u);
-        else wgmma_rs_n64<kBF16, 1>(dk, ds + 4 * kk, d_q, 1u);
+        const uint64_t d_do = make_desc(sDO + kk * 16 * 128, kBoxQ, 1024);
+        if constexpr (kD == 128) wgmma_rs_n128<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
+        else wgmma_rs_n64<kBF16, 1>(dv, pp + 4 * kk, d_do, 1u);
       }
       wgmma_commit();
-    };
-    if (reducer) {
-      const uint32_t a0 = smem_u32(sDS), b0 = sK + wg * kBoxKV;
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < kBwdN / 16; ++kk)
-        wgmma_ss_n64<kBF16, 1, 1>(dq, make_desc(a0 + kk * 16 * 128, 8192, 1024),
-                                  make_desc(b0 + kk * 16 * 128, kBoxKV, 1024), kk > 0 ? 1u : 0u);
-      wgmma_commit();
-      issue_dk();
-      wgmma_wait<1>();  // dV and dQ done, dK may still run
-    } else {
-      wgmma_fence();
-      issue_dk();
-      wgmma_wait<1>();  // dV done, dK may still run
-    }
-    fence_regs<kAcc>(dv);
-    fence_regs<16>(pp);
 
-    if (reducer) {
-      fence_regs<32>(dq);
-      const uint32_t bar_id = 2 + wg;
-      if (tid == 0) tma_store_wait_read<0>();  // the previous reduce has finished reading the staging tile
-      named_bar_sync(bar_id, 128);
-      // This thread holds dQ rows 16 w + g + 8 r (row % 8 = g) at columns 8 c + 2 t, 8 c + 2 t + 1.  Column 8 c + 2 t
-      // lies in box c / 4, 16-byte chunk j = 2 (c % 4) + t / 2 of its row, at byte 8 (t % 2) of the chunk; SW128
-      // stores chunk j at j ^ g.  Rows are 128 bytes, so the bank of a store depends on that chunk only, and one
-      // STS.64 of 16 lanes (g = 0..3 or 4..7, t = 0..3) needs 8 distinct chunks to be a single wavefront.  Storing
-      // every thread's chunk c = k at iteration k gives chunks {2 (k % 4), 2 (k % 4) + 1} ^ g: rows g and g ^ 1 meet,
-      // 2 wavefronts per half-warp.  A lane with odd g therefore stores c = k ^ 2 instead: its chunk is
-      // 2 (k % 4) ^ x with x = 4 (g % 2) ^ g ^ t / 2, and x takes all 8 values over the 16 lanes of either half-warp
-      // (g = 0..3: {0,1} {5,4} {2,3} {7,6}; g = 4..7: {4,5} {1,0} {6,7} {3,2}), so every STS.64 is 2 wavefronts, one
-      // per half-warp.  c = k ^ 2 (g % 2) runs over 0..7 once, so each of the 64 x 32 float2 slots is written once.
-      // The value is a register select between dq of chunks k and k ^ 2 (no dynamic register index).
-      const bool odd = g & 1;
-      const int x = (odd ? 4 : 0) ^ g ^ (t >> 1);
-      uint8_t* row = sDQ + (16 * w + g) * 128 + 8 * (t & 1);
+      // dS^T = P^T o (dP^T - delta) while dV runs
+      uint32_t ds[16];
 #pragma unroll
-      for (int k = 0; k < 8; ++k)
+      for (int c = 0; c < 8; ++c) {
+        const float2 dl = *reinterpret_cast<const float2*>(stat + kBwdM + 8 * c + 2 * t);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-          const int e = 4 * k + 2 * r, e2 = 4 * (k ^ 2) + 2 * r;
-          const float v0 = odd ? dq[e2] : dq[e], v1 = odd ? dq[e2 + 1] : dq[e + 1];
-          *reinterpret_cast<float2*>(row + (k >> 2) * kDQBox + r * 8 * 128 + ((2 * (k & 3) ^ x) << 4)) =
-              make_float2(v0 * p.scale, v1 * p.scale);
-        }
-      fence_proxy_async_smem();
-      named_bar_sync(bar_id, 128);
-      if (tid == 0) {
-        // deterministic mode: the fp32 adds into dq_acc[query head, q block] happen in key-block order.  Key
-        // block x visits Q block i iff i_begin(x) <= i < i_end(x) (neither depends on the query head); both
-        // bounds grow with x, so the key blocks that visit Q block i are one run x_min..x_max.  Without a band's
-        // lower edge x_min = 0; with one, x visits i iff 128 x + 127 >= 64 i + lo, i.e. x_min = max(0, q0 + lo) / 128
-        // (the last key block is cut at Sk, but if it is x_min and misses i, no key block sees i and nobody waits).
-        // The counter starts at 0, so the turn of key block x is (x - x_min) n_red + wg: x_min's first reducer
-        // never waits, and each later one waits for x - 1, which visits i too.  Lower key blocks are tickets of
-        // CTAs of the same (batch, K/V head) that started earlier (see the top of the kernel).  A CTA visits its
-        // (query head, Q block) pairs once each, head-major and in increasing Q block order like every other CTA,
-        // and only ever waits for a lower ticket; by induction over tickets (a CTA waits only for a lower ticket,
-        // which by hypothesis completes all its reductions) every wait ends, so waiting for our turn cannot
-        // deadlock.
-        int* turn = p.sem ? p.sem + ((int64_t)b * p.H + h) * nQ + (i_begin + it) : nullptr;
-        int x_min = 0;
-        if constexpr (kBand) x_min = max(0, q0 + p.lo) / kBwdN;
-        const int my_turn = (kb - x_min) * n_red + wg;
-        if (turn) {
-          while (ld_acquire_gpu(turn) != my_turn) __nanosleep(64);
-        }
-        tma_reduce_add_4d(&tmDQ, sDQ, wg * 64, h, q0, b);
-        tma_reduce_add_4d(&tmDQ, sDQ + kDQBox, wg * 64 + 32, h, q0, b);
-        tma_store_commit();  // one bulk group: the wait below covers both boxes
-        if (turn) {
-          tma_store_wait<0>();  // our reduction has been performed ...
-          __threadfence();
-          st_release_gpu(turn, my_turn + 1);  // ... next turn
+          const int e = 4 * c + 2 * r;
+          ds[2 * c + r] = pack2<kBF16>(s[e] * (dp[e] - dl.x), s[e + 1] * (dp[e + 1] - dl.y));
         }
       }
-    }
-    wgmma_wait<0>();  // dK done: ds may be rewritten, and Q of this stage is no longer read
-    fence_regs<kAcc>(dk);
-    fence_regs<16>(ds);
-    // Q, dO and the statistics of this stage are no longer read by this warp
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bars->q_empty[st]);
-    if (++it == n_it) it = 0, ++h;
-  }
-  if (reducer && tid == 0) tma_store_wait<0>();
+
+      // dS^T -> smem [128 keys][64 q] (SW128: 16-byte chunk j of row r at j ^ (r % 8)), double-buffered by step
+      // parity: the buffer written here was last read by the dQ and dK MMAs of step - 2.  Each reducing warpgroup's
+      // wgmma_wait<1> of step - 2 completes its dQ group (dV and dQ are the two oldest of its three groups), and that
+      // wait comes before the warpgroup reaches the barrier of step - 1, which this warpgroup has passed.  dK reads
+      // only this warpgroup's own 64 key rows, and its group was retired by this warpgroup's first wait of step - 1.
+      uint8_t* sDS = smem + L::kOffDS + (step & 1) * kBwdN * 128;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int kr = kr_lo + 8 * r;
+          *reinterpret_cast<uint32_t*>(sDS + kr * 128 + ((c ^ (kr & 7)) << 4) + 4 * t) = ds[2 * c + r];
+        }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 256);
+
+      // dQ[:, 64 wg .. 64 wg + 63] = dS K  (A = dS^T tile read MN-major, B = K tile read MN-major), then the next
+      // step's S^T, then dK += dS^T Q (A = this warpgroup's 64 rows of the dS^T tile read K-major, B = Q read
+      // MN-major).  Groups complete in issue order, so with S^T ahead of dK the next step's first wait retires S^T
+      // alone: dK and the next dP^T stay queued under the next P^T, and S^T and dK under the dQ staging below.
+      // dK reads dS^T from smem rather than as packed registers: those 16 registers would stay live through the
+      // staging, beside dq and the next S^T, and the staging would exceed the register budget.
+      // The next step's stage is step - 2's, which both warpgroups released in step - 1, before its barrier, so
+      // the loader can fill it and the wait ends.
+      const int st_next = st == kBwdStages - 1 ? 0 : st + 1;
+      const int ph_next = st_next == 0 ? ph ^ 1 : ph;
+      [[maybe_unused]] float dq[32];
+      fence_regs<kAcc>(dk);
+      wgmma_fence();
+      if constexpr (kRed) {
+        const uint32_t a0 = smem_u32(sDS), b0 = sK + wg * kBoxKV;
+#pragma unroll
+        for (int kk = 0; kk < kBwdN / 16; ++kk)
+          wgmma_ss_n64<kBF16, 1, 1>(dq, make_desc(a0 + kk * 16 * 128, 8192, 1024),
+                                    make_desc(b0 + kk * 16 * 128, kBoxKV, 1024), kk > 0 ? 1u : 0u);
+        wgmma_commit();
+      }
+      if constexpr (kNext) {
+        mbar_wait(&bars->q_full[st_next], ph_next);
+        fence_regs<32>(s);
+        issue_xt(s, sK, q_stage(st_next));
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kBwdM / 16; ++kk) {
+        const uint64_t d_ds = make_desc(smem_u32(sDS) + kw + kk * 32, 16, 1024);
+        const uint64_t d_q = make_desc(sQ + kk * 16 * 128, kBoxQ, 1024);
+        if constexpr (kD == 128) wgmma_ss_n128<kBF16, 0, 1>(dk, d_ds, d_q, 1u);
+        else wgmma_ss_n64<kBF16, 0, 1>(dk, d_ds, d_q, 1u);
+      }
+      wgmma_commit();
+      // dV and dQ done; the next S^T (if any) and dK may still run
+      if constexpr (kNext) wgmma_wait<2>();
+      else wgmma_wait<1>();
+      fence_regs<kAcc>(dv);
+      fence_regs<16>(pp);
+      // dP^T follows the staging: issued before it, its 32 accumulators would be live beside dq and push the
+      // staging over the register budget.
+
+      if constexpr (kRed) {
+        fence_regs<32>(dq);
+        const uint32_t bar_id = 2 + wg;
+        if (tid == 0) tma_store_wait_read<0>();  // the previous reduce has finished reading the staging tile
+        named_bar_sync(bar_id, 128);
+        // This thread holds dQ rows 16 w + g + 8 r (row % 8 = g) at columns 8 c + 2 t, 8 c + 2 t + 1.  Column
+        // 8 c + 2 t lies in box c / 4, 16-byte chunk j = 2 (c % 4) + t / 2 of its row, at byte 8 (t % 2) of the
+        // chunk; SW128 stores chunk j at j ^ g.  Rows are 128 bytes, so the bank of a store depends on that chunk
+        // only, and one STS.64 of 16 lanes (g = 0..3 or 4..7, t = 0..3) needs 8 distinct chunks to be a single
+        // wavefront.  Storing every thread's chunk c = k at iteration k gives chunks {2 (k % 4), 2 (k % 4) + 1} ^ g:
+        // rows g and g ^ 1 meet, 2 wavefronts per half-warp.  A lane with odd g therefore stores c = k ^ 2 instead:
+        // its chunk is 2 (k % 4) ^ x with x = 4 (g % 2) ^ g ^ t / 2, and x takes all 8 values over the 16 lanes of
+        // either half-warp (g = 0..3: {0,1} {5,4} {2,3} {7,6}; g = 4..7: {4,5} {1,0} {6,7} {3,2}), so every STS.64
+        // is 2 wavefronts, one per half-warp.  c = k ^ 2 (g % 2) runs over 0..7 once, so each of the 64 x 32 float2
+        // slots is written once.  The value is a register select between dq of chunks k and k ^ 2 (no dynamic
+        // register index).
+        const bool odd = g & 1;
+        const int x = (odd ? 4 : 0) ^ g ^ (t >> 1);
+        uint8_t* row = sDQ + (16 * w + g) * 128 + 8 * (t & 1);
+#pragma unroll
+        for (int k = 0; k < 8; ++k)
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int e = 4 * k + 2 * r, e2 = 4 * (k ^ 2) + 2 * r;
+            const float v0 = odd ? dq[e2] : dq[e], v1 = odd ? dq[e2 + 1] : dq[e + 1];
+            *reinterpret_cast<float2*>(row + (k >> 2) * kDQBox + r * 8 * 128 + ((2 * (k & 3) ^ x) << 4)) =
+                make_float2(v0 * p.scale, v1 * p.scale);
+          }
+        fence_proxy_async_smem();
+        named_bar_sync(bar_id, 128);
+        if (tid == 0) {
+          // deterministic mode: the fp32 adds into dq_acc[query head, q block] happen in key-block order.  Key
+          // block x visits Q block i iff i_begin(x) <= i < i_end(x) (neither depends on the query head); both
+          // bounds grow with x, so the key blocks that visit Q block i are one run x_min..x_max.  Without a band's
+          // lower edge x_min = 0; with one, x visits i iff 128 x + 127 >= 64 i + lo, i.e. x_min = max(0, q0 + lo) /
+          // 128 (the last key block is cut at Sk, but if it is x_min and misses i, no key block sees i and nobody
+          // waits).  The counter starts at 0, so the turn of key block x is (x - x_min) n_red + wg: x_min's first
+          // reducer never waits, and each later one waits for x - 1, which visits i too.  Lower key blocks are
+          // tickets of CTAs of the same (batch, K/V head) that started earlier (see the top of the kernel).  A CTA
+          // visits its (query head, Q block) pairs once each, head-major and in increasing Q block order like every
+          // other CTA, and only ever waits for a lower ticket; by induction over tickets (a CTA waits only for a
+          // lower ticket, which by hypothesis completes all its reductions) every wait ends, so waiting for our
+          // turn cannot deadlock.  The wait issues no wgmma; dK and the next S^T run on under it.
+          int* turn = p.sem ? p.sem + ((int64_t)b * p.H + h) * nQ + (i_begin + it) : nullptr;
+          int x_min = 0;
+          if constexpr (kBand) x_min = max(0, q0 + p.lo) / kBwdN;
+          const int my_turn = (kb - x_min) * n_red + wg;
+          if (turn) {
+            while (ld_acquire_gpu(turn) != my_turn) __nanosleep(64);
+          }
+          tma_reduce_add_4d(&tmDQ, sDQ, wg * 64, h, q0, b);
+          tma_reduce_add_4d(&tmDQ, sDQ + kDQBox, wg * 64 + 32, h, q0, b);
+          tma_store_commit();  // one bulk group: the wait below covers both boxes
+          if (turn) {
+            tma_store_wait<0>();  // our reduction has been performed ...
+            __threadfence();
+            st_release_gpu(turn, my_turn + 1);  // ... next turn
+          }
+        }
+      }
+
+      if constexpr (kNext) {
+        fence_regs<32>(dp);
+        issue_xt(dp, sV, do_stage(st_next));
+      } else {
+        wgmma_wait<0>();  // dK done
+        fence_regs<kAcc>(dk);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->q_empty[st]);
+      }
+      if (++it == n_it) it = 0, ++h;
+      st = st_next, ph = ph_next;
+    };
+
+    for (int step = 0; step < n_steps - 1; ++step) step_body(std::true_type(), step);
+    step_body(std::false_type(), n_steps - 1);
+    if (kRed && tid == 0) tma_store_wait<0>();
+  };
+  if constexpr (kD == 128) consume(std::true_type());
+  else if (wg == 0) consume(std::true_type());
+  else consume(std::false_type());
 
   // ---------------------------------------------------------- epilogue: dk_acc += scale*dK, dv_acc += dV
 #pragma unroll
