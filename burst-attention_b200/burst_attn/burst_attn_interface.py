@@ -321,6 +321,68 @@ def _lower_kw(lo):
     return {} if lo is None else {"lower": lo}
 
 
+# --------------------------------------------------------------------------- #
+# ALiBi: -slope |pos_q - pos_k| over positions of the full sequence
+# --------------------------------------------------------------------------- #
+def _check_alibi(alibi_slopes, q, heads_dim):
+    """flash-attn's ``alibi_slopes`` (fp32, ``(nheads,)`` or ``(batch, nheads)``, on q's device) -> an fp32 [B, H]
+    view (stride 0 over the batch for one row), or None."""
+    if alibi_slopes is None:
+        return None
+    B, H = q.shape[0], q.shape[heads_dim]
+    if not isinstance(alibi_slopes, torch.Tensor):
+        raise TypeError(f"alibi_slopes must be a torch.Tensor, got {type(alibi_slopes).__name__}")
+    if alibi_slopes.dtype != torch.float32:
+        raise TypeError(f"alibi_slopes must be float32, got {alibi_slopes.dtype}")
+    if alibi_slopes.device != q.device:
+        raise ValueError(f"alibi_slopes is on {alibi_slopes.device}, q on {q.device}")
+    if tuple(alibi_slopes.shape) not in ((H,), (B, H)):
+        raise ValueError(f"alibi_slopes must have shape ({H},) or ({B}, {H}), got {tuple(alibi_slopes.shape)}")
+    if not bool(torch.isfinite(alibi_slopes).all()):
+        raise ValueError("alibi_slopes must be finite")
+    s = alibi_slopes.detach().contiguous()
+    return s.unsqueeze(0).expand(B, H) if s.dim() == 1 else s
+
+
+def _positions(layout, W, rank, S):
+    """Full-sequence position of local token x of ``rank``'s shard (``S`` tokens), as a function, and the distance
+    between neighbouring tokens.  ``layout`` "local" is one device's view; its rank is the offset of row 0."""
+    if layout == "striped":
+        return (lambda x: x * W + rank), W
+    if layout == "zigzag":
+        h = S // 2
+        return (lambda x: (rank * h + x) if x < h else ((2 * W - 1 - rank) * h + x - h)), 1
+    if layout == "local":
+        return (lambda x: x + rank), 1
+    return (lambda x: rank * S + x), 1
+
+
+def _alibi_kw(alibi, q0, k0):
+    """Keyword for the chunk operators: the ALiBi of the launch whose rows start at local row q0 and keys at local
+    key k0.  alibi: (slopes, pos_q, pos_k, pstride) with the position functions of ``_positions`` (or None)."""
+    if alibi is None:
+        return {}
+    slopes, pos_q, pos_k, pstride = alibi
+    return {"alibi": (slopes, pos_q(q0) - pos_k(k0), pstride)}
+
+
+def _alibi_window(window, causal, alibi):
+    """A call with ALiBi runs the band launches (they know where their rows and keys sit), with the unwindowed band
+    when there is no window."""
+    if alibi is None or window is not None:
+        return window
+    return (None, 0 if causal else None)
+
+
+def _ring_alibi(slopes, layout, W, iq, jk, S):
+    """The ALiBi of the round that attends the Q shard of rank iq to the K/V shard of rank jk (or None)."""
+    if slopes is None:
+        return None
+    pos_q, pstride = _positions(layout, W, iq, S)
+    pos_k, _ = _positions(layout, W, jk, S)
+    return slopes, pos_q, pos_k, pstride
+
+
 class _BandForward:
     """The launches of a windowed forward, known up front for every round, and their first / last duties.  Skipped
     launches must not drop either: the state is started by the first launch only if it covers every row (otherwise
@@ -340,7 +402,7 @@ class _BandForward:
             self.o_acc.zero_()
             lse.fill_(float("-inf"))
 
-    def run(self, ops, launches, q, k, v, lse, out, scale, seq_dim, bias=None):
+    def run(self, ops, launches, q, k, v, lse, out, scale, seq_dim, bias=None, alibi=None):
         for q0, qn, k0, kn, lo, hi in launches:
             first = self.first and self.done == 0
             last = self.last and self.done == self.n - 1
@@ -348,7 +410,7 @@ class _BandForward:
             ops.fwd_chunk(rows(q), k.narrow(seq_dim, k0, kn), v.narrow(seq_dim, k0, kn),
                           None if self.o_acc is None else rows(self.o_acc), lse.narrow(2, q0, qn),
                           rows(out) if last else None, scale, hi is not None, 0 if hi is None else hi, first, last,
-                          seq_dim, **_bias_kw(bias, k0, kn), **_lower_kw(lo))
+                          seq_dim, **_bias_kw(bias, k0, kn), **_lower_kw(lo), **_alibi_kw(alibi, q0, k0))
             self.done += 1
 
     def finish(self, ops, out, seq_dim):
@@ -357,13 +419,13 @@ class _BandForward:
 
 
 def _bwd_band_run(ops, launches, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic,
-                  bias=None):
+                  bias=None, alibi=None):
     for q0, qn, k0, kn, lo, hi in launches:
         rows = lambda t: t.narrow(seq_dim, q0, qn)  # noqa: E731
         keys = lambda t: t.narrow(seq_dim, k0, kn)  # noqa: E731
         ops.bwd_chunk(rows(g), rows(q), keys(k), keys(v), delta.narrow(2, q0, qn), lse.narrow(2, q0, qn),
                       rows(dq_part), keys(dk_acc), keys(dv_acc), scale, hi is not None, 0 if hi is None else hi, seq_dim,
-                      deterministic, **_bias_kw(bias, k0, kn), **_lower_kw(lo))
+                      deterministic, **_bias_kw(bias, k0, kn), **_lower_kw(lo), **_alibi_kw(alibi, q0, k0))
 
 
 def _check_inputs(q, k, v, seq_dim):
@@ -401,7 +463,7 @@ def _fwd_dispatch(ops, mode, r, W, i, j, q, cur_k, cur_v, o_acc, lse, out, scale
 # --------------------------------------------------------------------------- #
 # forward ring (reference OpBurstAttn.forward :171-253, OpBurstAttnStrip.forward :411-493)
 # --------------------------------------------------------------------------- #
-def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None):
+def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None, alibi=None):
     """mode: "none" (non-causal) | "zigzag" | "striped".  Returns (out, lse[B,H,S] fp32).  With a ``window``
     (``_check_window``) the rounds run the band launches of ``_round_pieces`` for the shard ``layout`` instead.
 
@@ -410,8 +472,12 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None)
     cycle starts with is at the same time forwarded to the next node over the inter-node ring, where it starts
     the following cycle -- a prefetch with L rounds of kernel time to hide behind.  Unlike the reference no
     send-side copy is made: the cycle's starting block is never a receive target while it is in flight (two
-    inter-node buffers alternate)."""
+    inter-node buffers alternate).
+
+    ``alibi`` (fp32 slopes [B, H] from ``_check_alibi``) runs the band launches too, with the unwindowed band when
+    there is no window, so that every launch knows where its rows and keys sit in the full sequence."""
     ops = get_ops()
+    window = _alibi_window(window, mode != "none", alibi)
     ring, inter, _ = topo.rings()
     L, M, W, i = topo.L, topo.M, topo.W, topo.rank
     B, S, H = q.shape[0], q.shape[seq_dim], q.shape[3 - seq_dim]
@@ -446,7 +512,7 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None)
                 _fwd_dispatch(ops, mode, r, W, i, j, q, cur[0], cur[1], o_acc, lse, out, scale, seq_dim)
             else:  # a round whose shard lies outside every row's window launches nothing
                 band.run(ops, _fwd_band_launches(_round_pieces(layout, W, i, j, S, window)), q, cur[0], cur[1], lse,
-                         out, scale, seq_dim)
+                         out, scale, seq_dim, alibi=_ring_alibi(alibi, layout, W, i, j, S))
             if t != L - 1:
                 ring.wait()
                 cur = nxt
@@ -484,8 +550,10 @@ def _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, sca
         raise ValueError(mode)
 
 
-def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, deterministic, window=None, layout=None):
+def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, deterministic, window=None, layout=None,
+                   alibi=None):
     ops = get_ops()
+    window = _alibi_window(window, mode != "none", alibi)
     W, i = topo.W, topo.rank
     dev = q.device
     q, k, v, d_o, out = (t.contiguous() for t in (q, k, v, d_o, out))
@@ -506,7 +574,8 @@ def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, determini
             return
         dlt, g, qq, ls = bundle  # the bundle of rank j against the K/V at home: rows of j, keys of i
         _bwd_band_run(ops, _bwd_band_launches(_round_pieces(layout, W, j, i, S, window)), g, qq, k, v, dlt, ls,
-                      dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic)
+                      dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic,
+                      alibi=_ring_alibi(alibi, layout, W, j, i, S))
 
     bundle = [delta, d_o, q, lse.contiguous()]
     if W == 1:
@@ -620,9 +689,10 @@ def _bwd_rounds(ops, topo, round_kernel, bundle, q, seq_dim):
 
 # --------------------------------------------------------------------------- #
 def _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-             double_group, window_size=(-1, -1)):
+             double_group, window_size=(-1, -1), alibi_slopes=None):
     assert not causal or flash == "cuda", "Causal attention only supported for Flash v2"
     ctx.window = _check_window(window_size, causal)
+    ctx.alibi = _check_alibi(alibi_slopes, q, 2 if flash in ["cuda", "triton"] else 1)
     ctx.softmax_scale = 1 / math.sqrt(q.shape[-1]) if softmax_scale is None else softmax_scale
     ctx.flash = None if flash not in ["cuda", "triton"] else flash
     ctx.seq_dim = 1 if ctx.flash else 2
@@ -662,6 +732,9 @@ def _op_forward(ctx, q, k, v, mode, layout):
         if ctx.window is not None:
             raise NotImplementedError("window_size is not supported with host-resident (pinned CPU) operands; pass "
                                       "CUDA tensors")
+        if ctx.alibi is not None:
+            raise NotImplementedError("alibi_slopes is not supported with host-resident (pinned CPU) operands; pass "
+                                      "CUDA tensors")
         # host-resident operands (pinned CPU tensors, one rank): copies stream under the kernels (host_stream.py)
         from . import host_stream
         if not host_stream.is_host_call(q, k, v):
@@ -674,7 +747,7 @@ def _op_forward(ctx, q, k, v, mode, layout):
         ctx.save_for_backward(*saved)
         return o_host
     (qp, kp, vp), ctx.head_dim = _pad_head_dim(get_ops(), [q, k, v])
-    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, mode, ctx.topo, ctx.window, layout)
+    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, mode, ctx.topo, ctx.window, layout, ctx.alibi)
     ctx.mode, ctx.layout = mode, layout
     ctx.save_for_backward(qp, kp, vp, lse, out)
     return _unpad(out, ctx.head_dim)
@@ -685,12 +758,12 @@ def _op_backward(ctx, grad_output):
         from . import host_stream
         grads = host_stream.backward(grad_output, ctx.saved_tensors, ctx.softmax_scale, ctx.seq_dim,
                                      ctx.mode != "none", _l2_block(), ctx.deterministic)
-        return tuple(grads) + (None,) * 8
+        return tuple(grads) + (None,) * 9
     q, k, v, lse, out = ctx.saved_tensors
     (g,), _ = _pad_head_dim(get_ops(), [grad_output])
     dq, dk, dv = _ring_backward(g, q, k, v, out, lse, ctx.softmax_scale, ctx.seq_dim, ctx.mode, ctx.topo,
-                                ctx.deterministic, ctx.window, ctx.layout)
-    return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 8
+                                ctx.deterministic, ctx.window, ctx.layout, ctx.alibi)
+    return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 9
 
 
 class OpBurstAttn(torch.autograd.Function):
@@ -699,14 +772,16 @@ class OpBurstAttn(torch.autograd.Function):
     for Flash ("cuda"/"triton"):        q, k, v: [B, S, N, H]
     Each rank passes its own sequence shard: contiguous when non-causal, zigzag
     halves {i, 2W-1-i} when causal.  window_size: flash-attn's (left, right) sliding window over positions of
-    the full sequence (-1: unlimited side; causal forces right = 0).
+    the full sequence (-1: unlimited side; causal forces right = 0).  alibi_slopes: flash-attn's ALiBi, fp32
+    (nheads,) or (batch, nheads) per query head: the bias -slope |pos_q - pos_k| over the same positions.
     """
 
     @staticmethod
     def forward(ctx, q, k, v, softmax_scale=None, flash="cuda", causal=False, optimize_bwd_comm=False,
-                deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1)):
+                deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1),
+                alibi_slopes=None):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-                 double_group, window_size)
+                 double_group, window_size, alibi_slopes)
         return _op_forward(ctx, q, k, v, "zigzag" if causal else "none", "zigzag" if causal else "contiguous")
 
     @staticmethod
@@ -720,9 +795,10 @@ class OpBurstAttnStrip(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, q, k, v, softmax_scale=None, flash="cuda", causal=False, optimize_bwd_comm=False,
-                deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1)):
+                deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1),
+                alibi_slopes=None):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-                 double_group, window_size)
+                 double_group, window_size, alibi_slopes)
         return _op_forward(ctx, q, k, v, "striped" if causal else "none", "striped")
 
     @staticmethod
@@ -733,14 +809,14 @@ class OpBurstAttnStrip(torch.autograd.Function):
 def burst_attn_func_striped(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: float = None,
                             flash: str = "cuda", causal: bool = False, optimize_bwd_comm: bool = False,
                             deterministic: bool = False, process_group=None, double_group=[None, None],
-                            window_size=(-1, -1)):
+                            window_size=(-1, -1), alibi_slopes=None):
     return OpBurstAttnStrip.apply(q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic,
-                                  process_group, double_group, window_size)
+                                  process_group, double_group, window_size, alibi_slopes)
 
 
 def burst_attn_func(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: float = None,
                     flash: str = "cuda", causal: bool = False, optimize_bwd_comm: bool = False,
                     deterministic: bool = False, process_group=None, double_group=[None, None],
-                    window_size=(-1, -1)):
+                    window_size=(-1, -1), alibi_slopes=None):
     return OpBurstAttn.apply(q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic,
-                             process_group, double_group, window_size)
+                             process_group, double_group, window_size, alibi_slopes)

@@ -24,6 +24,13 @@ def _dims(t: torch.Tensor, seq_dim: int):
     return t.shape[0], t.shape[seq_dim], t.shape[3 - seq_dim], t.shape[3]
 
 
+def _alibi_args(alibi):
+    """(slopes fp32 [B, H], dist0, pstride) -> the C-ABI's (slopes, slopes_stride_b, dist0, pstride)."""
+    slopes, dist0, pstride = alibi
+    assert slopes.dim() == 2 and slopes.stride(1) == 1 and slopes.dtype == torch.float32
+    return slopes.data_ptr(), slopes.stride(0), int(dist0), int(pstride)
+
+
 class NativeOps:
     name = "sm90"
     tile_head_dims = (64, 128)  # head dims the tile kernels are built for; the drivers zero-pad others up
@@ -70,10 +77,12 @@ class NativeOps:
 
     # ---- forward round: fold chunk (k, v) into (o_acc, lse); on last write o_out
     def fwd_chunk(self, q, k, v, o_acc, lse, o_out, scale, causal, causal_offset, first, last, seq_dim, bias=None,
-                  lower=None):
+                  lower=None, alibi=None):
         """bias: optional fp32 [B|1, H, Sk] additive bias per key (expanded views with stride 0 over the batch are fine),
         indexed by the query head.  lower: optional lower edge of a band mask, key c visible to row a only if
-        c >= a + lower (None: no lower edge)."""
+        c >= a + lower (None: no lower edge).  alibi: optional ``(slopes, dist0, pstride)``, the bias
+        -slopes[b, h] |pstride (a - c) + dist0| with slopes fp32 [B, H] (stride 0 over the batch is fine); not
+        combined with ``bias``."""
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         flags = (_n.BA_FWD_FIRST if first else 0) | (_n.BA_FWD_LAST if last else 0)
@@ -81,7 +90,12 @@ class NativeOps:
         args = (_n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(bias), _n.t4(o_acc, seq_dim), _n.rs(lse),
                 _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale),
                 _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
-        if lower is None:
+        if alibi is not None:
+            assert bias is None, "ALiBi is not combined with a key bias"
+            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
+            rc = self.lib.ba_fwd_chunk_alibi(*args[:3], *args[4:-2], mask, args[-1], 0 if lower is None else int(lower),
+                                             *_alibi_args(alibi), flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        elif lower is None:
             rc = self.lib.ba_fwd_chunk_gqa(*args, flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
         else:
             args = args[:-2] + (args[-2] | _n.BA_MASK_LOWER, args[-1], int(lower))
@@ -103,8 +117,8 @@ class NativeOps:
 
     # ---- backward round: accumulate into fp32 dq_acc / dk_acc / dv_acc
     def bwd_chunk(self, d_o, q, k, v, delta, lse, dq_acc, dk_acc, dv_acc, scale, causal, causal_offset, seq_dim,
-                  deterministic=False, bias=None, lower=None):
-        """lower: as in fwd_chunk."""
+                  deterministic=False, bias=None, lower=None, alibi=None):
+        """lower, alibi: as in fwd_chunk."""
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         e0 = self._t0(q.device)
@@ -112,7 +126,12 @@ class NativeOps:
                 _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv,
                 D, float(scale), _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
         tail = (1 if deterministic else 0, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
-        if lower is None:
+        if alibi is not None:
+            assert bias is None, "ALiBi is not combined with a key bias"
+            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
+            rc = self.lib.ba_bwd_chunk_alibi(*args[:6], *args[7:-2], mask, args[-1], 0 if lower is None else int(lower),
+                                             *_alibi_args(alibi), *tail)
+        elif lower is None:
             rc = self.lib.ba_bwd_chunk_gqa(*args, *tail)
         else:
             args = args[:-2] + (args[-2] | _n.BA_MASK_LOWER, args[-1], int(lower))

@@ -7,10 +7,10 @@ that its ring op never calls; here the three wrappers run the same sm_90a tile k
 the strides; nothing is unpacked or copied on the way in).
 
 ``bias`` (the Triton copy's additive attention bias, lao.py:102-105,155-173): the per-KEY form -- shape
-``(batch | 1, nheads, 1, seqlen_k)``, the reference's "vector" bias, e.g. an ALiBi row or a key-padding mask of
--inf -- runs in the tile kernels (forward: one extra K = 16 step on the tensor core per score tile; backward: a
-per-thread scalar in the exponent's FMA).  The "matrix" form ``(.., seqlen_q, seqlen_k)`` is not supported (at the
-sequence lengths this path is built for it does not fit memory) and raises.  As in the reference no gradient
+``(batch | 1, nheads, 1, seqlen_k)``, the reference's "vector" bias, e.g. a key-padding mask of -inf (ALiBi has its
+own argument, ``alibi_slopes``) -- runs in the tile kernels (forward: one extra K = 16 step on the tensor core per
+score tile; backward: a per-thread scalar in the exponent's FMA).  The "matrix" form ``(.., seqlen_q, seqlen_k)`` is
+not supported (at the sequence lengths this path is built for it does not fit memory) and raises.  As in the reference no gradient
 flows into the bias.
 
 Grouped-query / multi-query attention as in flash-attn: ``flash_attn_func`` and ``flash_attn_kvpacked_func`` accept
@@ -22,6 +22,10 @@ Sliding-window (local) attention as in flash-attn: ``window_size=(left, right)``
 ``i`` sees key ``j`` iff ``i + Sk - Sq - left <= j <= i + Sk - Sq + right`` (the bottom-right alignment of ``causal``,
 which forces ``right = 0``).  The tile kernels skip the key tiles outside each row block's band.  A row that sees no
 key returns 0 and gets no gradient.
+
+ALiBi as in flash-attn: ``alibi_slopes``, fp32 ``(nheads,)`` or ``(batch, nheads)`` indexed by the query head, adds
+``-slope |i + Sk - Sq - j|`` to the score of query row ``i`` and key ``j`` (bottom-right aligned).  It combines with
+``causal``, ``window_size`` and grouped-query attention, not with ``bias``; no gradient flows into the slopes.
 """
 from __future__ import annotations
 
@@ -29,9 +33,9 @@ import math
 
 import torch
 
-from .burst_attn_interface import (_band, _BandForward, _bwd_band_launches, _bwd_band_run, _bwd_round,
-                                   _check_window, _fwd_band_launches, _fwd_round, _fwd_round_needs_state,
-                                   _pad_head_dim, _unpad)
+from .burst_attn_interface import (_alibi_window, _band, _BandForward, _bwd_band_launches, _bwd_band_run,
+                                   _bwd_round, _check_alibi, _check_window, _fwd_band_launches, _fwd_round,
+                                   _fwd_round_needs_state, _pad_head_dim, _positions, _unpad)
 from .chunk_ops import get_ops
 
 __all__ = ["flash_attn_func", "flash_attn_kvpacked_func", "flash_attn_qkvpacked_func"]
@@ -57,17 +61,27 @@ def _window_pieces(window, Sq, Sk):
     return [] if b is None else [(0, Sq, 0, Sk) + b]
 
 
-def _local_forward(q, k, v, causal, softmax_scale, bias=None, window=None):
+def _local_alibi(slopes, Sq, Sk):
+    """The ALiBi of a local call (bottom-right aligned: row i sits at position i + Sk - Sq), or None."""
+    if slopes is None:
+        return None
+    pos_q, _ = _positions("local", 1, Sk - Sq, Sq)
+    pos_k, _ = _positions("local", 1, 0, Sk)
+    return slopes, pos_q, pos_k, 1
+
+
+def _local_forward(q, k, v, causal, softmax_scale, bias=None, window=None, alibi=None):
     ops = get_ops()
     scale = softmax_scale or 1.0 / math.sqrt(q.shape[-1])
     (qp, kp, vp), D = _pad_head_dim(ops, [q, k, v])
     B, Sq, H = qp.shape[0], qp.shape[1], qp.shape[2]
     out = torch.empty(qp.shape, dtype=qp.dtype, device=qp.device)
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=qp.device)
+    window = _alibi_window(window, causal, alibi)
     if window is not None:
         launches = _fwd_band_launches(_window_pieces(window, Sq, kp.shape[1]))
         band = _BandForward([launches], qp, lse, Sq)
-        band.run(ops, launches, qp, kp, vp, lse, out, scale, 1, bias)
+        band.run(ops, launches, qp, kp, vp, lse, out, scale, 1, bias, _local_alibi(alibi, Sq, kp.shape[1]))
         band.finish(ops, out, 1)
         return out, lse, scale, (qp, kp, vp), D
     o_acc = torch.empty(qp.shape, dtype=torch.float32, device=qp.device) if _fwd_round_needs_state(kp, 1) else None
@@ -75,7 +89,7 @@ def _local_forward(q, k, v, causal, softmax_scale, bias=None, window=None):
     return out, lse, scale, (qp, kp, vp), D
 
 
-def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, deterministic=False, window=None):
+def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, deterministic=False, window=None, alibi=None):
     ops = get_ops()
     (g,), _ = _pad_head_dim(ops, [do])
     g, out = g.contiguous(), out.contiguous()
@@ -84,9 +98,10 @@ def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, determin
     ops.delta(out, g, delta, 1)
     f32 = dict(dtype=torch.float32, device=qp.device)
     dq, dk, dv = torch.zeros(qp.shape, **f32), torch.zeros(kp.shape, **f32), torch.zeros(vp.shape, **f32)
+    window = _alibi_window(window, causal, alibi)
     if window is not None:
         _bwd_band_run(ops, _bwd_band_launches(_window_pieces(window, Sq, kp.shape[1])), g, qp, kp, vp, delta, lse, dq,
-                      dk, dv, scale, 1, deterministic, bias)
+                      dk, dv, scale, 1, deterministic, bias, _local_alibi(alibi, Sq, kp.shape[1]))
         return dq, dk, dv
     _bwd_round(ops, g, qp, kp, vp, delta, lse, dq, dk, dv, scale, causal, kp.shape[1] - Sq, 1, deterministic, bias)
     return dq, dk, dv
@@ -103,6 +118,13 @@ def _check(bias, *ts):
         assert t.stride(-1) == 1, "the head_dim axis must be contiguous"
 
 
+def _alibi(alibi_slopes, bias, q):
+    slopes = _check_alibi(alibi_slopes, q, 2)
+    if slopes is not None and bias is not None:
+        raise NotImplementedError("alibi_slopes together with a per-key bias is not supported")
+    return slopes
+
+
 def _check_heads(q, k):
     hq, hkv = q.shape[2], k.shape[2]
     assert hkv > 0 and hq % hkv == 0, f"nheads ({hq}) must be a multiple of nheads_k ({hkv})"
@@ -113,13 +135,14 @@ class FlashAttnFunc(torch.autograd.Function):
     (reference :1122-1168)."""
 
     @staticmethod
-    def forward(ctx, q, k, v, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1)):
+    def forward(ctx, q, k, v, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1), alibi_slopes=None):
         _check(bias, q, k, v)
         _check_heads(q, k)
         ctx.bias = _key_bias(bias, q, k)
         ctx.window = _check_window(window_size, causal)
+        ctx.alibi = _alibi(alibi_slopes, bias, q)
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, k, v, causal, softmax_scale, ctx.bias,
-                                                                          ctx.window)
+                                                                          ctx.window, ctx.alibi)
         ctx.save_for_backward(*saved, out, lse)
         ctx.causal = causal
         return _unpad(out, ctx.head_dim)
@@ -128,9 +151,9 @@ class FlashAttnFunc(torch.autograd.Function):
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
         dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
-                                     window=ctx.window)
+                                     window=ctx.window, alibi=ctx.alibi)
         return (_cast(dq, qp, ctx.head_dim), _cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim), None, None, None,
-                None)
+                None, None)
 
 
 class FlashAttnKVPackedFunc(torch.autograd.Function):
@@ -138,13 +161,14 @@ class FlashAttnKVPackedFunc(torch.autograd.Function):
     (reference :1073-1119)."""
 
     @staticmethod
-    def forward(ctx, q, kv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1)):
+    def forward(ctx, q, kv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1), alibi_slopes=None):
         _check(bias, q, kv)
         _check_heads(q, kv[:, :, 0])
         ctx.bias = _key_bias(bias, q, kv[:, :, 0])
         ctx.window = _check_window(window_size, causal)
+        ctx.alibi = _alibi(alibi_slopes, bias, q)
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, kv[:, :, 0], kv[:, :, 1], causal,
-                                                                          softmax_scale, ctx.bias, ctx.window)
+                                                                          softmax_scale, ctx.bias, ctx.window, ctx.alibi)
         ctx.save_for_backward(*saved, out, lse)
         ctx.causal = causal
         return _unpad(out, ctx.head_dim)
@@ -153,21 +177,22 @@ class FlashAttnKVPackedFunc(torch.autograd.Function):
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
         dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
-                                     window=ctx.window)
+                                     window=ctx.window, alibi=ctx.alibi)
         dkv = torch.stack([_cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim)], dim=2)
-        return _cast(dq, qp, ctx.head_dim), dkv, None, None, None, None
+        return _cast(dq, qp, ctx.head_dim), dkv, None, None, None, None, None
 
 
 class FlashAttnQKVPackedFunc(torch.autograd.Function):
     """qkv: (batch, seqlen, 3, nheads, headdim)  (reference :1021-1070)."""
 
     @staticmethod
-    def forward(ctx, qkv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1)):
+    def forward(ctx, qkv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1), alibi_slopes=None):
         _check(bias, qkv)
         ctx.bias = _key_bias(bias, qkv[:, :, 0], qkv[:, :, 1])
         ctx.window = _check_window(window_size, causal)
+        ctx.alibi = _alibi(alibi_slopes, bias, qkv[:, :, 0])
         out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal,
-                                                                          softmax_scale, ctx.bias, ctx.window)
+                                                                          softmax_scale, ctx.bias, ctx.window, ctx.alibi)
         ctx.save_for_backward(*saved, out, lse)
         ctx.causal = causal
         return _unpad(out, ctx.head_dim)
@@ -176,9 +201,9 @@ class FlashAttnQKVPackedFunc(torch.autograd.Function):
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
         dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
-                                     window=ctx.window)
+                                     window=ctx.window, alibi=ctx.alibi)
         dqkv = torch.stack([_cast(t, qp, ctx.head_dim) for t in (dq, dk, dv)], dim=2)
-        return dqkv, None, None, None, None
+        return dqkv, None, None, None, None, None
 
 
 flash_attn_func = FlashAttnFunc.apply

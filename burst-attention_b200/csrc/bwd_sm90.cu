@@ -70,16 +70,15 @@ extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_t
                            mask_mode, causal_offset, 0, flags, dtype, stream);
 }
 
-extern "C" int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
-                                 ba_rowstat lse, ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc,
-                                 ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
-                                 int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
-                                 void* stream) {
-  using namespace ba;
+namespace ba {
+
+// ba_bwd_chunk_band and ba_bwd_chunk_alibi after their argument checks (slopes: ALiBi, else null)
+static int bwd_chunk_run(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
+                         ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq,
+                         int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset,
+                         int lower_offset, const float* slopes, int64_t slopes_stride_b, int64_t dist0, int pstride,
+                         int flags, int dtype, void* stream) {
   int rc;
-  if ((rc = check_band_args("ba_bwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset, &lower_offset,
-                            dtype)))
-    return rc;
   BA_REQUIRE(d_o.ptr && q.ptr && k.ptr && v.ptr && delta.ptr && lse.ptr, "ba_bwd_chunk: null input");
   BA_REQUIRE(dq_acc.ptr && dk_acc.ptr && dv_acc.ptr && aligned16(dq_acc, 4) && aligned16(dk_acc, 4) &&
                  aligned16(dv_acc, 4),
@@ -122,6 +121,38 @@ extern "C" int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
       return BA_ERR_CUDA;
     }
   }
+  p.slopes = slopes, p.slopes_sb = slopes_stride_b, p.dist0 = dist0, p.pstride = pstride;
+  if (slopes) return launch_bwd_alibi(dtype, D, (mask_mode & BA_MASK_LOWER) != 0, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
   if (mask_mode & BA_MASK_LOWER) return launch_bwd_band(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
   return launch_bwd<false>(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
+}
+
+}  // namespace ba
+
+extern "C" int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
+                                 ba_rowstat lse, ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc,
+                                 ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
+                                 int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
+                                 void* stream) {
+  int rc;
+  if ((rc = ba::check_band_args("ba_bwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+                                &lower_offset, dtype)))
+    return rc;
+  return ba::bwd_chunk_run(d_o, q, k, v, delta, lse, key_bias, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H_kv, D, scale,
+                           mask_mode, causal_offset, lower_offset, nullptr, 0, 0, 1, flags, dtype, stream);
+}
+
+extern "C" int ba_bwd_chunk_alibi(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
+                                  ba_rowstat lse, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq,
+                                  int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset,
+                                  int lower_offset, const float* slopes, int64_t slopes_stride_b, int64_t dist0,
+                                  int pstride, int flags, int dtype, void* stream) {
+  int rc;
+  if ((rc = ba::check_alibi_args("ba_bwd_chunk_alibi", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+                                 &lower_offset, slopes, slopes_stride_b, pstride, dtype)))
+    return rc;
+  ba_rowstat none = {nullptr, 0, 0};
+  return ba::bwd_chunk_run(d_o, q, k, v, delta, lse, none, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H_kv, D, scale,
+                           mask_mode, causal_offset, lower_offset, slopes, slopes_stride_b, dist0, pstride, flags,
+                           dtype, stream);
 }

@@ -42,6 +42,8 @@
 // Band mask (kBand, sliding-window attention): key c is visible to row a iff a + lo <= c (and c <= a + causal_off
 // when causal).  A key block then visits the Q blocks [i_begin, i_end) only, and P^T gets the band's lower edge.
 // kBand = false is the kernel without a lower edge (bwd_sm90.cu); kBand = true lives in bwd_band_sm90.cu.
+//
+// ALiBi (kAlibi, bwd_alibi_kernel in bwd_alibi_sm90.cu): P^T gets -slope |pstride (q - c) + dist0| (see bwd_chunk_body).
 #pragma once
 #include <math.h>
 #include <stdlib.h>
@@ -78,7 +80,22 @@ struct BwdParams {
   int* sem;     // deterministic mode: [B][H][nQ] turn counters ordering the dQ reductions by key block; else null
   int* ticket;  // deterministic mode: [B][H/G] key-block tickets (a CTA's key block = the order in which it STARTED)
   int lo;       // kBand: key c is visible to row a only if c >= a + lo
+  // kAlibi (appended, so the fields above keep their offsets): row a and key c get the bias -slope |d| with the
+  // exact integer distance d = pstride (a - c) + dist0; slope = slopes[b * slopes_sb + h] (query head)
+  const float* slopes;
+  int64_t slopes_sb;
+  int64_t dist0;
+  int pstride;
 };
+
+// ALiBi over the tile of the 64 rows from q0 and the 128 keys from k0: +1 or -1 when d has that sign (or is 0) on
+// the whole tile, 0 when the tile crosses d = 0
+__device__ __forceinline__ int alibi_tile_sign(int q0, int k0, const BwdParams& p) {
+  const int64_t base = (int64_t)p.pstride * (q0 - k0) + p.dist0;
+  if (base - (int64_t)p.pstride * (kBwdN - 1) >= 0) return 1;
+  if (base + (int64_t)p.pstride * (kBwdM - 1) <= 0) return -1;
+  return 0;
+}
 
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
@@ -117,11 +134,14 @@ struct BwdLayout {
   static_assert(kOffDQ % 1024 == 0, "SW128 dQ staging boxes need 1 KiB alignment");
 };
 
-template <bool kBF16, int kD, bool kBand>
-__global__ void __launch_bounds__(kBwdThreads, 1)
-bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                 const __grid_constant__ CUtensorMap tmDQ, const BwdParams p) {
+// The kernel body; bwd_chunk_kernel (kAlibi = false) and bwd_alibi_kernel (kAlibi = true, no key bias) wrap it.
+// ALiBi: on a tile where d has one sign s, -slope |d| = -slope s (pstride (q - k0) + dist0) + s slope pstride (c - k0):
+// the loader folds the per-row term into the row's lse2 (it is per tile: k0 is the CTA's), and the per-key term sits
+// where the key bias goes.  On a tile that crosses d = 0, every |d| is below 192 pstride, exact in fp32, and the bias
+// is formed per element.
+template <bool kBF16, int kD, bool kBand, bool kAlibi>
+__device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                                               const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();  // SWIZZLE_128B atoms need a 1 KiB-aligned base
@@ -190,6 +210,12 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     int st = 0, ph = 0;  // stage of this step (step % kBwdStages) and its phase ((step / kBwdStages) & 1)
     for (int step = 0; step < n_steps; ++step) {
       const int q0 = (i_begin + it) * kBwdM;
+      [[maybe_unused]] float slope2 = 0.f;
+      [[maybe_unused]] int sg = 0;
+      if constexpr (kAlibi) {
+        slope2 = __ldg(p.slopes + (int64_t)b * p.slopes_sb + h) * kLog2e;
+        sg = alibi_tile_sign(q0, k0, p);
+      }
       mbar_wait(&bars->q_empty[st], ph ^ 1);
       // row statistics of this Q block (lane handles rows lane, lane + 32): lse in log2 units, delta
       float* stat = sStat + st * 2 * kBwdM;
@@ -202,7 +228,12 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
           dl = __ldg(p.delta + (int64_t)b * p.dl_sb + (int64_t)h * p.dl_sh + row);
           if (l == -INFINITY) l = INFINITY;
         }
-        stat[lane + 32 * j] = l * kLog2e;
+        if constexpr (kAlibi) {  // + slope s (pstride (q - k0) + dist0), the exact integer converted once
+          const float x = (float)(sg * ((int64_t)p.pstride * (row - k0) + p.dist0));
+          stat[lane + 32 * j] = fmaf(slope2, x, l * kLog2e);
+        } else {
+          stat[lane + 32 * j] = l * kLog2e;
+        }
         stat[kBwdM + lane + 32 * j] = dl;
       }
       __syncwarp();
@@ -283,7 +314,20 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const int q0 = (i_begin + it) * kBwdM;
       const uint32_t sQ = q_stage(st), sDO = do_stage(st);
       const float* stat = sStat + st * 2 * kBwdM;
-      if (it == 0) {
+      // ALiBi: the bias relative to the row term the loader folded into lse2 is ma |ka[r] + kc (q - q0)|.  One-sign
+      // tile s: ma = s slope, ka = pstride (c - k0), kc = 0.  Crossing tile: ma = -slope, ka + kc (q - q0) = d, with
+      // ka = pstride (q0 + 2 t - c) + dist0 (small: the 32-bit sum wraps, and its true value fits) and kc = pstride.
+      [[maybe_unused]] float ma = 0.f, kc = 0.f, ka[2];
+      if constexpr (kAlibi) {
+        const float slope2 = __ldg(p.slopes + (int64_t)b * p.slopes_sb + h) * kLog2e;
+        const int sg = alibi_tile_sign(q0, k0, p);
+        ma = sg > 0 ? slope2 : -slope2;
+        kc = sg == 0 ? (float)p.pstride : 0.f;
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          ka[r] = sg == 0 ? (float)(int)((unsigned)p.pstride * (unsigned)(q0 + 2 * t - keys[r]) + (unsigned)p.dist0)
+                          : (float)(p.pstride * (keys[r] - k0));
+      } else if (it == 0) {
 #pragma unroll
         for (int r = 0; r < 2; ++r)
           bias2[r] = (p.bias && keys[r] < p.Sk)
@@ -306,8 +350,16 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
           const int e = 4 * c + 2 * r;
-          float p0 = ex2(fmaf(s[e], scale_log2, bias2[r] - l2.x));
-          float p1 = ex2(fmaf(s[e + 1], scale_log2, bias2[r] - l2.y));
+          float p0, p1;
+          if constexpr (kAlibi) {
+            const float x0 = fmaf(ma, fabsf(fmaf(kc, (float)(8 * c), ka[r])), -l2.x);
+            const float x1 = fmaf(ma, fabsf(fmaf(kc, (float)(8 * c + 1), ka[r])), -l2.y);
+            p0 = ex2(fmaf(s[e], scale_log2, x0));
+            p1 = ex2(fmaf(s[e + 1], scale_log2, x1));
+          } else {
+            p0 = ex2(fmaf(s[e], scale_log2, bias2[r] - l2.x));
+            p1 = ex2(fmaf(s[e + 1], scale_log2, bias2[r] - l2.y));
+          }
           if (keys[r] >= p.Sk) p0 = p1 = 0.f;
           if (need_mask) {
             const int q = q0 + 8 * c + 2 * t;
@@ -517,6 +569,23 @@ bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   }
 }
 
+template <bool kBF16, int kD, bool kBand>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+bwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                 const __grid_constant__ CUtensorMap tmDQ, const BwdParams p) {
+  bwd_chunk_body<kBF16, kD, kBand, false>(tmQ, tmK, tmV, tmDO, tmDQ, p);
+}
+
+// ALiBi instantiations: bwd_alibi_sm90.cu
+template <bool kBF16, int kD, bool kBand>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+bwd_alibi_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                 const __grid_constant__ CUtensorMap tmDQ, const BwdParams p) {
+  bwd_chunk_body<kBF16, kD, kBand, true>(tmQ, tmK, tmV, tmDO, tmDQ, p);
+}
+
 // the kernel of one (dtype, head dim) for this TU's kBand; bwd_sm90.cu launches kBand = false,
 // bwd_band_sm90.cu (launch_bwd_band) kBand = true
 template <bool kBand>
@@ -536,5 +605,9 @@ inline int launch_bwd(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMa
 
 int launch_bwd_band(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                     const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream);
+// bwd_alibi_sm90.cu: the ALiBi kernel of (dtype, head dim, band)
+int launch_bwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                     const CUtensorMap& tmV, const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p,
+                     cudaStream_t stream);
 
 }  // namespace ba

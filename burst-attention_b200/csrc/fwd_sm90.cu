@@ -25,15 +25,14 @@ extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_row
                            causal_offset, 0, flags, dtype, stream);
 }
 
-extern "C" int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
-                                 ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D,
-                                 float scale, int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
-                                 void* stream) {
-  using namespace ba;
+namespace ba {
+
+// ba_fwd_chunk_band and ba_fwd_chunk_alibi after their argument checks (slopes: ALiBi, else null)
+static int fwd_chunk_run(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
+                         ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
+                         int mask_mode, int causal_offset, int lower_offset, const float* slopes,
+                         int64_t slopes_stride_b, int64_t dist0, int pstride, int flags, int dtype, void* stream) {
   int rc;
-  if ((rc = check_band_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset, &lower_offset,
-                            dtype)))
-    return rc;
   BA_REQUIRE(q.ptr && k.ptr && v.ptr && lse.ptr, "ba_fwd_chunk: null q/k/v/lse");
   const bool first = flags & BA_FWD_FIRST, last = flags & BA_FWD_LAST;
   BA_REQUIRE(!last || o_out.ptr, "ba_fwd_chunk: BA_FWD_LAST needs o_out");
@@ -65,8 +64,38 @@ extern "C" int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
   p.store_lowp = last ? 1 : 0;
   p.lo = lower_offset;
   p.bias = key_bias.ptr, p.bias_sb = key_bias.stride_b, p.bias_sh = key_bias.stride_h;
+  p.slopes = slopes, p.slopes_sb = slopes_stride_b, p.dist0 = dist0, p.pstride = pstride;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bias = key_bias.ptr != nullptr;
+  if (slopes) return launch_fwd_alibi(dtype, D, (mask_mode & BA_MASK_LOWER) != 0, tmQ, tmK, tmV, p, st);
   if (mask_mode & BA_MASK_LOWER) return launch_fwd_band(dtype, D, bias, tmQ, tmK, tmV, p, st);
   return launch_fwd<false>(dtype, D, bias, tmQ, tmK, tmV, p, st);
+}
+
+}  // namespace ba
+
+extern "C" int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
+                                 ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D,
+                                 float scale, int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
+                                 void* stream) {
+  int rc;
+  if ((rc = ba::check_band_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+                                &lower_offset, dtype)))
+    return rc;
+  return ba::fwd_chunk_run(q, k, v, key_bias, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode,
+                           causal_offset, lower_offset, nullptr, 0, 0, 1, flags, dtype, stream);
+}
+
+extern "C" int ba_fwd_chunk_alibi(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse,
+                                  ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
+                                  int mask_mode, int causal_offset, int lower_offset, const float* slopes,
+                                  int64_t slopes_stride_b, int64_t dist0, int pstride, int flags, int dtype,
+                                  void* stream) {
+  int rc;
+  if ((rc = ba::check_alibi_args("ba_fwd_chunk_alibi", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+                                 &lower_offset, slopes, slopes_stride_b, pstride, dtype)))
+    return rc;
+  ba_rowstat none = {nullptr, 0, 0};
+  return ba::fwd_chunk_run(q, k, v, none, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset,
+                           lower_offset, slopes, slopes_stride_b, dist0, pstride, flags, dtype, stream);
 }

@@ -25,6 +25,10 @@
 // first row's lowest visible key, so tiles entirely below the band of all its rows are never loaded, and each
 // consumer warpgroup works on its own sub-range of them.  kBand = false is the kernel without a lower edge; its
 // instantiations live in fwd_sm90.cu, the kBand = true ones in fwd_band_sm90.cu.
+//
+// ALiBi (kAlibi, fwd_alibi_kernel in fwd_alibi_sm90.cu): the score of row a and key c gets -slope |pstride (a - c) +
+// dist0|, formed from exact integer distances relative to each row's reference (alibi_dref); tiles and masks are
+// unchanged.
 #pragma once
 #include <math.h>
 #include <stdlib.h>
@@ -58,6 +62,12 @@ struct FwdParams {
   int load_state;
   int store_lowp;
   int lo;  // kBand: key c is visible to row a only if c >= a + lo
+  // kAlibi (appended, so the fields above keep their offsets): row a and key c get the bias -slope |d| with the
+  // exact integer distance d = pstride (a - c) + dist0; slope = slopes[b * slopes_sb + h] (query head)
+  const float* slopes;
+  int64_t slopes_sb;
+  int64_t dist0;
+  int pstride;
 };
 
 struct __align__(8) FwdBarriers {
@@ -95,10 +105,32 @@ __device__ __forceinline__ int fwd_trip_count(int r0, const FwdParams& p) {
 // the host clamps lo to <= Sk, so r0 + lo does not overflow)
 __device__ __forceinline__ int fwd_first_tile(int r0, const FwdParams& p) { return max(0, r0 + p.lo) / kBlockN; }
 
-template <bool kBF16, int kD, bool kBias, bool kBand>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
+// ALiBi: the smallest |d| of row a over the view's keys 0 .. Sk-1 (0 if d changes sign).  The kernel runs the row's
+// softmax relative to the bias -slope dref, so that far from d = 0 its fp32 scores stay small: a pair's score gets
+// -slope (|d| - dref), an exact integer times the slope, and only lse carries -slope dref.  A carried state lowers
+// dref (alibi_carried_ref) so that its lse, taken to the row's reference, stays small too.
+__device__ __forceinline__ int64_t alibi_dref(int a, const FwdParams& p) {
+  const int64_t hi = (int64_t)p.pstride * a + p.dist0, lo = hi - (int64_t)p.pstride * (p.Sk - 1);
+  return max((int64_t)0, max(lo, -hi));
+}
+
+// ALiBi with a carried state of lse m0 (log2 units): the reference is lowered to at most max(0, -m0) / slope, so that
+// the carried state in the row's frame, m0 + slope dref, is at most max(m0, 0) and its fp32 rounding is that of m0
+// itself rather than of slope dref.  Any dref <= the smallest |d| is exact (every |d| - dref stays a non-negative
+// integer); keys it leaves far below the carried state only underflow to 0, as they would anyway.
+__device__ __forceinline__ int64_t alibi_carried_ref(int64_t dref, float m0, float slope2) {
+  if (slope2 > 0.f) {
+    const float cap = fmaxf(0.f, -m0) / slope2;
+    if (cap < (float)dref) return (int64_t)cap;
+  }
+  return dref;
+}
+
+// The kernel body; fwd_chunk_kernel (kAlibi = false) and fwd_alibi_kernel (kAlibi = true, no key bias) wrap it.
+template <bool kBF16, int kD, bool kBias, bool kBand, bool kAlibi>
+__device__ __forceinline__ void fwd_chunk_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                                               const FwdParams& p) {
+  static_assert(!(kBias && kAlibi), "ALiBi is not combined with the key bias");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();      // SWIZZLE_128B atoms need a 1 KiB-aligned base
@@ -206,6 +238,14 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     lo_limit[1] = rows[1] + p.lo;
   }
   const int lo_limit_max = max(lo_limit[0], lo_limit[1]);
+  // ALiBi: slope in log2 units, and each row's reference distance (alibi_dref)
+  float slope2 = 0.f;
+  int64_t dref[2] = {0, 0};
+  if constexpr (kAlibi) {
+    slope2 = __ldg(p.slopes + (int64_t)b * p.slopes_sb + h) * kLog2e;
+    dref[0] = alibi_dref(rows[0], p);
+    dref[1] = alibi_dref(rows[1], p);
+  }
 
   float o[kOReg];
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};  // l: this thread's partial row sums
@@ -218,6 +258,10 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const float lse_prev = p.lse[(int64_t)b * p.lse_sb + (int64_t)h * p.lse_sh + rows[r]];
       if (lse_prev != -INFINITY) {
         m[r] = lse_prev * kLog2e;
+        if constexpr (kAlibi) {
+          dref[r] = alibi_carried_ref(dref[r], m[r], slope2);
+          m[r] += slope2 * (float)dref[r];
+        }
         l[r] = t == 0 ? 1.f : 0.f;  // counted once per row
       }
       const float* src = p.o_acc + (int64_t)b * p.oacc_sb + (int64_t)rows[r] * p.oacc_ss + (int64_t)h * p.oacc_sh;
@@ -263,6 +307,40 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
             sc[4 * c + 2 * r] = fmaf(sc[4 * c + 2 * r], scale_log2, bb.x);
             sc[4 * c + 2 * r + 1] = fmaf(sc[4 * c + 2 * r + 1], scale_log2, bb.y);
           }
+        }
+      } else if constexpr (kAlibi) {
+        // d = pstride (a - c) + dist0 over this group's 64 rows x 128 keys; j = c - key0 (0..127)
+        const int64_t base = (int64_t)p.pstride * (row0 + wg * 64 - key0) + p.dist0;
+        const int64_t dmin = base - (int64_t)p.pstride * (kBlockN - 1), dmax = base + (int64_t)p.pstride * 63;
+        const float pf = (float)p.pstride;
+        if (dmin >= 0 || dmax <= 0) {
+          // one sign s: |d| - dref = x_row - s pstride j, with the exact integer x_row = s (pstride (a - key0) +
+          // dist0) - dref >= 0.  Score += -slope x_row (per row) + s slope pstride j (per key).
+          const int sg = dmin >= 0 ? 1 : -1;
+          float rowb[2];
+#pragma unroll
+          for (int r = 0; r < 2; ++r)
+            rowb[r] = -slope2 * (float)(sg * ((int64_t)p.pstride * (rows[r] - key0) + p.dist0) - dref[r]);
+          const float ks = sg > 0 ? slope2 * pf : -slope2 * pf, kt = ks * (float)(2 * t);
+#pragma unroll
+          for (int c = 0; c < 16; ++c)
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+              sc[4 * c + e] = fmaf(sc[4 * c + e], scale_log2, rowb[e >> 1] + fmaf(ks, (float)(8 * c + (e & 1)), kt));
+        } else {
+          // the tile crosses d = 0, so every |d| here is below 256 pstride and exact in fp32
+          float dr[2], dreff[2];
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            dr[r] = (float)((int64_t)p.pstride * (rows[r] - key0 - 2 * t) + p.dist0);
+            dreff[r] = slope2 * (float)dref[r];
+          }
+#pragma unroll
+          for (int c = 0; c < 16; ++c)
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+              sc[4 * c + e] = fmaf(-slope2, fabsf(fmaf(-pf, (float)(8 * c + (e & 1)), dr[e >> 1])),
+                                   fmaf(sc[4 * c + e], scale_log2, dreff[e >> 1]));
         }
       } else {
 #pragma unroll
@@ -348,7 +426,13 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const int row = rows[r];
     if (row >= p.Sq) continue;
     const float inv_l = lr > 0.f ? 1.f / lr : 0.f;
-    if (t == 0) p.lse[(int64_t)b * p.lse_sb + (int64_t)h * p.lse_sh + row] = lr > 0.f ? (m[r] + lg2(lr)) * kLn2 : -INFINITY;
+    if constexpr (kAlibi) {  // back from the row's reference to the absolute bias
+      if (t == 0)
+        p.lse[(int64_t)b * p.lse_sb + (int64_t)h * p.lse_sh + row] =
+            lr > 0.f ? (m[r] + lg2(lr) - slope2 * (float)dref[r]) * kLn2 : -INFINITY;
+    } else {
+      if (t == 0) p.lse[(int64_t)b * p.lse_sb + (int64_t)h * p.lse_sh + row] = lr > 0.f ? (m[r] + lg2(lr)) * kLn2 : -INFINITY;
+    }
     if (p.store_lowp) {
       uint16_t* dst = reinterpret_cast<uint16_t*>(p.o_out) + (int64_t)b * p.oout_sb + (int64_t)row * p.oout_ss +
                       (int64_t)h * p.oout_sh + 2 * t;
@@ -362,6 +446,21 @@ fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         *reinterpret_cast<float2*>(dst + 8 * c) = make_float2(o[4 * c + 2 * r] * inv_l, o[4 * c + 2 * r + 1] * inv_l);
     }
   }
+}
+
+template <bool kBF16, int kD, bool kBias, bool kBand>
+__global__ void __launch_bounds__(kFwdThreads, 1)
+fwd_chunk_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
+  fwd_chunk_body<kBF16, kD, kBias, kBand, false>(tmQ, tmK, tmV, p);
+}
+
+// ALiBi instantiations: fwd_alibi_sm90.cu
+template <bool kBF16, int kD, bool kBand>
+__global__ void __launch_bounds__(kFwdThreads, 1)
+fwd_alibi_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
+  fwd_chunk_body<kBF16, kD, false, kBand, true>(tmQ, tmK, tmV, p);
 }
 
 // the kernel of one (dtype, head dim, bias) for this TU's kBand; fwd_sm90.cu launches kBand = false,
@@ -387,5 +486,8 @@ inline int launch_fwd(int dtype, int D, bool bias, const CUtensorMap& tmQ, const
 
 int launch_fwd_band(int dtype, int D, bool bias, const CUtensorMap& tmQ, const CUtensorMap& tmK,
                     const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream);
+// fwd_alibi_sm90.cu: the ALiBi kernel of (dtype, head dim, band)
+int launch_fwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
+                     const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream);
 
 }  // namespace ba

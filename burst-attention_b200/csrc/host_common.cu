@@ -105,6 +105,19 @@ int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int 
   return BA_OK;
 }
 
+int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
+                     int causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
+                     int dtype) {
+  int rc;
+  if ((rc = check_band_args(fn, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset, lower_offset, dtype)))
+    return rc;
+  BA_REQUIRE(slopes, "%s: null ALiBi slopes", fn);
+  BA_REQUIRE((reinterpret_cast<uintptr_t>(slopes) & 3) == 0, "%s: ALiBi slopes must be 4-byte aligned", fn);
+  BA_REQUIRE(slopes_stride_b >= 0, "%s: ALiBi slopes batch stride %lld is negative", fn, (long long)slopes_stride_b);
+  BA_REQUIRE(pstride >= 1, "%s: ALiBi position stride %d must be >= 1", fn, pstride);
+  return BA_OK;
+}
+
 }  // namespace ba
 
 #ifdef BA_SELFTEST_LIB
@@ -113,7 +126,8 @@ extern "C" const char* ba_selftest_last_error(void) { return ba::g_err; }
 extern "C" const char* ba_last_error(void) { return ba::g_err; }
 // 201: grouped-query attention (ba_fwd_chunk_gqa, ba_bwd_chunk_gqa); 202: band masks (ba_fwd_chunk_band,
 // ba_bwd_chunk_band)
-extern "C" int ba_version(void) { return 202; }
+// 203: ALiBi (ba_fwd_chunk_alibi, ba_bwd_chunk_alibi)
+extern "C" int ba_version(void) { return 203; }
 extern "C" int ba_device_check(void) {
   int dev = 0;
   BA_CHECK_CUDA(cudaGetDevice(&dev));

@@ -59,4 +59,9 @@ int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int
 int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
                     int causal_offset, int* lower_offset, int dtype);
 
+// The same for the ALiBi entry points: check_band_args, plus the slopes (non-null, batch stride >= 0) and pstride >= 1.
+int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
+                     int causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
+                     int dtype);
+
 }  // namespace ba

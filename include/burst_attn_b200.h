@@ -106,6 +106,16 @@ int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_b
                       ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
                       int causal_offset, int lower_offset, int flags, int dtype, void* stream);
 
+/* ALiBi (linear position bias): ba_fwd_chunk_band without a key bias, plus the bias -slope |d| added to the scores of
+ * row i and key j (before the softmax), with the distance d = pstride (i - j) + dist0 counted in exact integers.
+ * slopes: fp32, one per query head, of batch b at slopes + b * slopes_stride_b (0: one row for every batch).  A ring
+ * passes dist0 = the full-sequence position of row 0 minus that of key 0, and pstride = the distance in the full
+ * sequence between neighbouring rows (1, or W for a striped shard).  pstride >= 1.                               */
+int ba_fwd_chunk_alibi(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse, ba_tensor4 o_out,
+                       int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset,
+                       int lower_offset, const float* slopes, int64_t slopes_stride_b, int64_t dist0, int pstride,
+                       int flags, int dtype, void* stream);
+
 /* delta[b,h,s] = sum_d O[b,s,h,d] * dO[b,s,h,d]  (burst_attn_interface.py:272-278) */
 int ba_bwd_delta(ba_tensor4 o, ba_tensor4 d_o, ba_rowstat delta, int B, int S, int H, int D, int dtype,
                  void* stream);
@@ -139,6 +149,13 @@ int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, 
                       ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq,
                       int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset, int lower_offset,
                       int flags, int dtype, void* stream);
+
+/* ALiBi: ba_bwd_chunk_band without a key bias, plus the bias of ba_fwd_chunk_alibi.  No gradient flows into the
+ * slopes.                                                                                                        */
+int ba_bwd_chunk_alibi(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
+                       ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv,
+                       int D, float scale, int mask_mode, int causal_offset, int lower_offset, const float* slopes,
+                       int64_t slopes_stride_b, int64_t dist0, int pstride, int flags, int dtype, void* stream);
 
 /* dst[b,s,h,d] (dtype) = src[b,s,h,d] (fp32); used once per backward to hand the
  * fp32 gradient accumulators back in the input dtype.                              */
