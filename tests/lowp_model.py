@@ -241,6 +241,20 @@ def oracle_chain(q, ks, vs, do, scale, masks, biases=None):
     lse_b = torch.where(torch.isinf(lse), torch.full_like(lse, float("inf")), lse)  # dead rows: P = 0
     dq = torch.zeros(q.shape, dtype=torch.float64)
     dks, dvs = [], []
+    for c in range(n):
+        dqc, dk, dv = orc.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, modes[c], key_bias=cpu(biases[c]))
+        dq += dqc
+        dks.append(_group_sum(dk, Hkv))
+        dvs.append(_group_sum(dv, Hkv))
+    return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs,
+                **error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, [cpu(b) for b in biases], Hkv))
+
+
+def error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, biases, Hkv):
+    """The comparator's error scales of one fp64 chain (``oracle_chain``): dict(mag, rss, e32).  CPU tensors; kx / vx
+    per chunk at the query heads; lse_b the final lse with +inf for dead rows; ``biases[c]``: None, a key bias
+    [B|1,H,Sk] or a pair bias [B,H,Sq,Sk], in natural units."""
+    n = len(kx)
     # Per gradient row, two error scales no 16-bit model run reproduces by itself:
     # rss: the root sum of squares of the row's terms (P V for O, P dO for dV, dS K scale for dQ, dS Q scale for dK).
     #   A 16-bit rounding moves each term by at most u/2 of itself, so where a row's terms cancel (sum_k dS = 0
@@ -258,14 +272,11 @@ def oracle_chain(q, ks, vs, do, scale, masks, biases=None):
     dd = n2(o.double() * dod).sqrt().permute(0, 2, 1)  # [B,H,Sq]
     dq_d = torch.zeros(q.shape[:3], dtype=torch.float64)
     for c in range(n):
-        dqc, dk, dv = orc.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, modes[c], key_bias=cpu(biases[c]))
-        dq += dqc
-        dks.append(_group_sum(dk, Hkv))
-        dvs.append(_group_sum(dv, Hkv))
         kd, vd = kx[c].double(), vx[c].double()
         s = torch.einsum("bqhd,bkhd->bhqk", qd, kd) * scale
         if biases[c] is not None:
-            s = s + cpu(biases[c]).double().unsqueeze(2)
+            b = biases[c].double()
+            s = s + (b if b.dim() == 4 else b.unsqueeze(2))
         p = torch.exp(s - lse_b.unsqueeze(-1))
         vis = visible(q.shape[1], kd.shape[1], masks[c])
         if vis is not None:
@@ -287,13 +298,13 @@ def oracle_chain(q, ks, vs, do, scale, masks, biases=None):
     nrm = lambda ts: max(float(t.double().norm(dim=-1).max()) for t in ts)  # noqa: E731
     nq, ndo, nk, nv = nrm([q]), nrm([do]), nrm(kx), nrm(vx)
     mag = dict(dq=abs(scale) * ndo * nv * nk, dk=abs(scale) * ndo * nv * nq, dv=ndo)
-    return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs, mag=mag, rss=rss,
-                e32=dict(dq=e32_dq, dk=torch.cat(e32_dk, 1)))
+    return dict(mag=mag, rss=rss, e32=dict(dq=e32_dq, dk=torch.cat(e32_dk, 1)))
 
 
 def scores_absmax(q, ks, scale, masks, biases=None):
     """[B,H,Sq]: per row, the largest ``sum_d |q_d k_d| scale + |bias|`` over the keys the row sees in any chunk --
-    the magnitude the fp32 score arithmetic works at, which bounds its rounding error."""
+    the magnitude the fp32 score arithmetic works at, which bounds its rounding error.  ``biases[c]``: None, a key
+    bias [B|1,H,Sk] or a pair bias [B,H,Sq,Sk]."""
     n = len(ks)
     biases = biases or [None] * n
     q = q.detach().cpu().double().abs()
@@ -302,14 +313,17 @@ def scores_absmax(q, ks, scale, masks, biases=None):
     for c in range(n):
         k = _kv_heads(ks[c].detach().cpu(), H).double().abs()
         a = torch.einsum("bqhd,bkhd->bhqk", q, k) * abs(scale)
+        pair = biases[c] is not None and biases[c].dim() == 4
         if biases[c] is not None:
             bb = biases[c].detach().cpu().double().abs()
-            a = a + torch.where(torch.isinf(bb), torch.zeros_like(bb), bb).unsqueeze(2)
+            bb = torch.where(torch.isinf(bb), torch.zeros_like(bb), bb)
+            a = a + (bb if pair else bb.unsqueeze(2))
         vis = visible(q.shape[1], k.shape[1], masks[c])
         if vis is not None:
             a = a.masked_fill(~vis, 0.0)
         if biases[c] is not None:
-            a = a.masked_fill(torch.isinf(biases[c].detach().cpu()).unsqueeze(2).expand_as(a), 0.0)
+            inf = torch.isinf(biases[c].detach().cpu())
+            a = a.masked_fill((inf if pair else inf.unsqueeze(2)).expand_as(a), 0.0)
         out = torch.maximum(out, a.amax(-1))
     return out
 

@@ -136,3 +136,10 @@ def check_alibi_case(job, got):
     if m is not None:
         a = a.masked_fill(~m, 0.0)
     lm.assert_lse(f"lse[{job['id']}]", got["lse"], lse, a.amax(-1))
+    # per (b, s, h) row against the 16-bit model (lowp_alibi) of the whole sequence as one chunk: d = a - c
+    import lowp_alibi as la
+    al = [(ao.as_bh(_slopes(job), q.shape[0]).contiguous(), 0, 1)]
+    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], [job["mask"]], al)
+    absmax = la.absmax_prefix(x["q"], x["ks"], x["scale"], [job["mask"]], al)[-1]
+    lm.assert_api_within_model(job["id"], got, la.oracle_alibi_chain(*args), la.lowp_alibi_chain(*args),
+                               job["case"]["dtype"], absmax)
