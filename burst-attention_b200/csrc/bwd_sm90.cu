@@ -135,7 +135,7 @@ extern "C" int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
                                  int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
                                  void* stream) {
   int rc;
-  if ((rc = ba::check_band_args("ba_bwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+  if ((rc = ba::check_band_args("ba_bwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, &causal_offset,
                                 &lower_offset, dtype)))
     return rc;
   return ba::bwd_chunk_run(d_o, q, k, v, delta, lse, key_bias, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H_kv, D, scale,
@@ -148,7 +148,7 @@ extern "C" int ba_bwd_chunk_alibi(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba
                                   int lower_offset, const float* slopes, int64_t slopes_stride_b, int64_t dist0,
                                   int pstride, int flags, int dtype, void* stream) {
   int rc;
-  if ((rc = ba::check_alibi_args("ba_bwd_chunk_alibi", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+  if ((rc = ba::check_alibi_args("ba_bwd_chunk_alibi", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, &causal_offset,
                                  &lower_offset, slopes, slopes_stride_b, pstride, dtype)))
     return rc;
   ba_rowstat none = {nullptr, 0, 0};

@@ -79,7 +79,7 @@ extern "C" int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
                                  float scale, int mask_mode, int causal_offset, int lower_offset, int flags, int dtype,
                                  void* stream) {
   int rc;
-  if ((rc = ba::check_band_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+  if ((rc = ba::check_band_args("ba_fwd_chunk", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, &causal_offset,
                                 &lower_offset, dtype)))
     return rc;
   return ba::fwd_chunk_run(q, k, v, key_bias, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode,
@@ -92,7 +92,7 @@ extern "C" int ba_fwd_chunk_alibi(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_t
                                   int64_t slopes_stride_b, int64_t dist0, int pstride, int flags, int dtype,
                                   void* stream) {
   int rc;
-  if ((rc = ba::check_alibi_args("ba_fwd_chunk_alibi", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, causal_offset,
+  if ((rc = ba::check_alibi_args("ba_fwd_chunk_alibi", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, &causal_offset,
                                  &lower_offset, slopes, slopes_stride_b, pstride, dtype)))
     return rc;
   ba_rowstat none = {nullptr, 0, 0};

@@ -89,15 +89,20 @@ int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int
 }
 
 int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                    int causal_offset, int* lower_offset, int dtype) {
+                    int* causal_offset, int* lower_offset, int dtype) {
   const int mm = *mask_mode;
   BA_REQUIRE((mm & ~(BA_MASK_CAUSAL | BA_MASK_LOWER)) == 0, "%s: bad mask mode %d", fn, mm);
   int rc;
   if ((rc = check_chunk_args(fn, B, Sq, Sk, H, H_kv, D, scale, mm & BA_MASK_CAUSAL, dtype))) return rc;
-  if (!(mm & BA_MASK_LOWER)) return BA_OK;
-  BA_REQUIRE(!(mm & BA_MASK_CAUSAL) || *lower_offset <= causal_offset,
+  BA_REQUIRE(!(mm & BA_MASK_LOWER) || !(mm & BA_MASK_CAUSAL) || *lower_offset <= *causal_offset,
              "%s: band lower_offset %d is above its causal_offset %d (no key would be visible)", fn, *lower_offset,
-             causal_offset);
+             *causal_offset);
+  // The kernels add the causal offset to row and key indices in 32-bit arithmetic.  An offset >= Sk - 1 shows every
+  // key to every row and one <= -Sq shows none, so clamping it into [-Sq, Sk] changes no mask and keeps those sums in
+  // range.  A lower edge at or below the causal one stays there: both clamps below are monotone, and a clamped lower
+  // edge is at most Sk.
+  *causal_offset = *causal_offset > Sk ? Sk : *causal_offset < -Sq ? -Sq : *causal_offset;
+  if (!(mm & BA_MASK_LOWER)) return BA_OK;
   // a lower edge at or below key 0 for every row (lower_offset <= 1 - Sq) masks nothing: run the kernel without one;
   // one at or above Sk masks every key of every row, as lower_offset = Sk does (and row + Sk cannot overflow)
   if (*lower_offset <= 1 - Sq) *mask_mode = mm & ~BA_MASK_LOWER;
@@ -106,7 +111,7 @@ int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int 
 }
 
 int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                     int causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
+                     int* causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
                      int dtype) {
   int rc;
   if ((rc = check_band_args(fn, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset, lower_offset, dtype)))

@@ -53,15 +53,17 @@ inline bool aligned16(const ba_tensor4& t, int esize) {
 int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
                      int dtype);
 
-// The same for the band entry points, whose mask_mode is a set of BA_MASK_CAUSAL and BA_MASK_LOWER bits.  On
-// success it normalises the band: a lower edge that masks nothing is dropped from *mask_mode, and *lower_offset is
-// clamped to Sk.
+// The same for the band entry points, whose mask_mode is a set of BA_MASK_CAUSAL and BA_MASK_LOWER bits; every
+// forward and backward entry point ends up here.  On success it normalises the masks without changing which keys
+// are visible: *causal_offset is clamped into [-Sq, Sk] (beyond either end it shows every key or none, and the
+// kernels' 32-bit index sums with it stay in range), a lower edge that masks nothing is dropped from *mask_mode, and
+// *lower_offset is clamped to Sk -- still at or below the clamped causal offset.
 int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                    int causal_offset, int* lower_offset, int dtype);
+                    int* causal_offset, int* lower_offset, int dtype);
 
 // The same for the ALiBi entry points: check_band_args, plus the slopes (non-null, batch stride >= 0) and pstride >= 1.
 int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                     int causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
+                     int* causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
                      int dtype);
 
 }  // namespace ba

@@ -1,11 +1,17 @@
 """Sliding-window (band) attention on the GPU: the tile kernels' band mask, the flash_attn_* wrappers and the ring.
 
-* Chunk kernels: ``NativeOps.fwd_chunk`` / ``bwd_chunk`` with a band ``("band", lo, hi)`` -- key b visible to row a iff
-  a + lo <= b <= a + hi -- over chains of K/V chunks with carried state, against the fp64 oracle and the 16-bit model
-  (``lowp_model``): bands inside one tile, across 128-key tiles and 64-row blocks, narrower than a warpgroup's 64
-  rows, beyond Sk (dead rows), ragged Sq / Sk, head dim 64 and 128, bf16 and fp16, GQA, a key bias, carried state.
-  Dead rows must give O = 0, dQ = 0 and lse = -inf exactly, keys no row sees dK = dV = 0 exactly, and deterministic
-  mode must be bitwise reproducible.  Three faults of the band's lower edge injected into the model must be rejected.
+* Chunk kernels: every case of ``lowp_band.BAND_SWEEP`` runs ``NativeOps.fwd_chunk`` / ``bwd_chunk`` with a band
+  ``("band", lo, hi)`` -- key b visible to row a iff a + lo <= b <= a + hi -- over a chain of K/V chunks with carried
+  state, straight through the C-ABI, against the fp64 oracle scaled by the error of the 16-bit model (``lowp_model``):
+  the fp32 (o_acc, lse) state after every non-last chunk, O, lse, dQ, dK and dV per (b, s, h) row.  The sweep puts the
+  band's lower edge on every phase of the forward's 128-key tiles and warpgroups and on the backward's i_end and
+  need_lo boundaries, reaches CTAs and key blocks with no work, the host's lower-edge clamps, the deterministic mode's
+  turn counters from a key block x_min >= 1, chains of up to 16 chunks with rows dead, revived and blind in the last
+  chunk, key biases that mask the band's edge or all of it, ragged Sq / Sk, head dim 64 and 128, bf16 and fp16, GQA
+  and MQA, and the flash, [B,H,S,D] and batch-strided layouts.  Dead rows must give O = 0, dQ = 0 and lse = -inf
+  exactly, keys no row sees dK = dV = 0 exactly, and deterministic mode must be bitwise reproducible.  Every fault of
+  ``lowp_band.BAND_MUTANTS`` injected into the model is rejected on the same inputs.
+* Causal offsets at the ends of the C-ABI's int range give what the nearest in-range offsets (Sk, -Sq) give.
 * ``flash_attn_func`` / ``_kvpacked_func`` / ``_qkvpacked_func`` with ``window_size``, causal and not, Sq != Sk, with
   BA_L2_BLOCK = 256 so that rows whose first visible key block is not block 0 start their state in later launches.
 * The ring at W = 2, 4 and 8 on one device (``ring_band`` over ``ring_harness``), flat and hierarchical, in all three shard layouts.
@@ -25,6 +31,7 @@ from burst_attn.chunk_ops import NativeOps  # noqa: E402
 
 BF16, FP16 = torch.bfloat16, torch.float16
 lowp_band.install()  # lowp_model's model, oracle chain and comparator take the band masks below
+_BY_ID = {c["id"]: c for c in lowp_band.BAND_SWEEP}
 
 
 def _kw(m, bias):
@@ -40,10 +47,29 @@ def _kw(m, bias):
     return hi is not None, 0 if hi is None else hi, kw
 
 
-def native_chain(x, det_runs=2):
+def _kernel_layout(t, layout):
+    """A view of the logical [B,S,H,D] tensor t as the kernels see it in this case (values unchanged)."""
+    if layout == "normal":
+        return t.transpose(1, 2).contiguous()  # [B,H,S,D] storage
+    if layout == "bstride":
+        big = torch.zeros((2 * t.shape[0],) + tuple(t.shape[1:]), device=t.device, dtype=t.dtype)
+        big[::2] = t
+        return big[::2]
+    return t
+
+
+def _logical(t, layout):
+    return t.transpose(1, 2) if layout == "normal" else t
+
+
+def native_chain(x, layout="flash", det_runs=2):
+    """The band kernels on one case: (result dict like lowp_chain's, [deterministic (dq, dks, dvs)])."""
     ops = NativeOps()
-    q, do, ks, vs = x["q"], x["do"], x["ks"], x["vs"]
-    B, Sq, H = q.shape[:3]
+    sd = 2 if layout == "normal" else 1
+    q, do = _kernel_layout(x["q"], layout), _kernel_layout(x["do"], layout)
+    ks = [_kernel_layout(k, layout) for k in x["ks"]]
+    vs = [_kernel_layout(v, layout) for v in x["vs"]]
+    B, Sq, H = x["q"].shape[:3]
     n = len(ks)
     out = torch.empty_like(q)
     lse = torch.empty(B, H, Sq, device="cuda", dtype=torch.float32)
@@ -51,11 +77,11 @@ def native_chain(x, det_runs=2):
     states = []
     for c, m in enumerate(x["masks"]):
         causal, off, kw = _kw(m, x["biases"][c])
-        ops.fwd_chunk(q, ks[c], vs[c], o_acc, lse, out, x["scale"], causal, off, c == 0, c == n - 1, 1, **kw)
+        ops.fwd_chunk(q, ks[c], vs[c], o_acc, lse, out, x["scale"], causal, off, c == 0, c == n - 1, sd, **kw)
         if c < n - 1:
-            states.append((o_acc.clone(), lse.clone()))
+            states.append((_logical(o_acc, layout).clone(), lse.clone()))
     delta = torch.empty(B, H, Sq, device="cuda", dtype=torch.float32)
-    ops.delta(out, do, delta, 1)
+    ops.delta(out, do, delta, sd)
 
     def backward(det):
         dq = torch.zeros(q.shape, device="cuda", dtype=torch.float32)
@@ -64,49 +90,16 @@ def native_chain(x, det_runs=2):
             causal, off, kw = _kw(m, x["biases"][c])
             dk = torch.zeros(ks[c].shape, device="cuda", dtype=torch.float32)
             dv = torch.zeros(vs[c].shape, device="cuda", dtype=torch.float32)
-            ops.bwd_chunk(do, q, ks[c], vs[c], delta, lse, dq, dk, dv, x["scale"], causal, off, 1, deterministic=det,
+            ops.bwd_chunk(do, q, ks[c], vs[c], delta, lse, dq, dk, dv, x["scale"], causal, off, sd, deterministic=det,
                           **kw)
-            dks.append(dk)
-            dvs.append(dv)
-        return dq, dks, dvs
+            dks.append(_logical(dk, layout))
+            dvs.append(_logical(dv, layout))
+        return _logical(dq, layout), dks, dvs
 
     dq, dks, dvs = backward(False)
     dets = [backward(True) for _ in range(det_runs)]
     torch.cuda.synchronize()
-    return dict(o=out, lse=lse, states=states, dq=dq, dk=dks, dv=dvs), dets
-
-
-def _case(sq, chunks, D=128, dtype=BF16, bias=None, H=2, Hkv=None, tag=""):
-    """chunks: [(Sk, lo, hi)]; the case id carries the bands (it seeds the inputs)."""
-    ch = "+".join(f"{sk}b{lo}_{hi}" for sk, lo, hi in chunks)
-    c = lm._case(sq, [(sk, None) for sk, _, _ in chunks], D, dtype, bias=bias, H=H, Hkv=Hkv, tag=f"band_{tag}{ch}_")
-    c["bands"] = [("band", lo, hi) for _, lo, hi in chunks]
-    return c
-
-
-CASES = [
-    _case(257, [(257, -5, 0)]),                      # causal window of 6 keys: inside one tile
-    _case(257, [(257, -100, 0)], 64, FP16),          # crosses 128-key tiles and 64-row blocks
-    _case(383, [(383, -30, 30)]),                    # two-sided, narrower than a warpgroup's 64 rows
-    _case(383, [(383, 0, 0)], 64, BF16),             # the diagonal only
-    _case(255, [(513, 129, 200)], 128, FP16),        # above the diagonal, Sq != Sk
-    _case(129, [(257, 200, None)]),                  # lower edge only; rows from 57 on see nothing (beyond Sk)
-    _case(130, [(1, -3, 2)], 64, FP16),              # one key
-    _case(65, [(300, -64, 63)], 128, BF16),          # ragged
-    _case(200, [(500, 150, 290)], 128, BF16, H=4, Hkv=2),   # GQA
-    _case(200, [(333, -40, 40)], 64, FP16, H=4, Hkv=1),     # MQA
-    _case(257, [(257, -70, 10)], 128, BF16, bias="randn"),  # key bias with a window
-    _case(129, [(257, -64, 128)], 64, FP16, bias="edge_inf"),
-    # carried state: views of one windowed problem, chunk offsets shifted by the chunk's start
-    _case(200, [(128, 0 - 60, 0), (128, -128 - 60, -128), (100, -256 - 60, -256)], 128, BF16, tag="chain_"),
-    _case(129, [(64, 300, None), (128, -64, 0), (200, -190, -100)], 64, FP16, tag="dead1st_"),
-]
-
-
-def _inputs(case):
-    x = lm.make_inputs(case, "cuda")
-    x["masks"] = case["bands"]
-    return x
+    return dict(o=_logical(out, layout), lse=lse, states=states, dq=dq, dk=dks, dv=dvs), dets
 
 
 def _check_dead(x, got, ref):
@@ -131,33 +124,83 @@ def _absmax(x):
             for c in range(len(x["ks"]))]
 
 
-@pytest.mark.parametrize("case", CASES, ids=[c["id"] for c in CASES])
-def test_band_chunks_within_model(case):
-    x = _inputs(case)
-    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], x["biases"])
-    got, dets = native_chain(x)
-    model, ref = lm.lowp_chain(*args), lm.oracle_chain(*args)
-    lm.assert_chain_within_model(case["id"], got, ref, model, case["dtype"], _absmax(x))
+def _args(x):
+    return (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], x["biases"])
+
+
+def _check_chain(name, x, got, dets, dtype, model=None, ref=None):
+    """got / dets of native_chain within the model, dead rows and unseen keys exact, deterministic runs bitwise equal
+    and within the model."""
+    model = lm.lowp_chain(*_args(x)) if model is None else model
+    ref = lm.oracle_chain(*_args(x)) if ref is None else ref
+    lm.assert_chain_within_model(name, got, ref, model, dtype, _absmax(x))
     _check_dead(x, got, ref)
     (dq0, dk0, dv0), (dq1, dk1, dv1) = dets
     assert torch.equal(dq0, dq1) and all(torch.equal(a, b) for a, b in zip(dk0 + dv0, dk1 + dv1)), \
         "deterministic mode is not bitwise reproducible with a band"
-    lm.assert_chain_within_model(case["id"] + " deterministic", dict(got, dq=dq0, dk=dk0, dv=dv0), ref, model,
-                                 case["dtype"], _absmax(x))
+    lm.assert_chain_within_model(name + " deterministic", dict(got, dq=dq0, dk=dk0, dv=dv0), ref, model, dtype,
+                                 _absmax(x))
 
 
-MUTANT_CASE = _case(383, [(383, -100, 20)], 128, BF16, tag="mutant_")
+@pytest.mark.parametrize("case", lowp_band.BAND_SWEEP, ids=[c["id"] for c in lowp_band.BAND_SWEEP])
+def test_band_chunks_within_model(case):
+    x = lowp_band.make_band_inputs(case, "cuda")
+    got, dets = native_chain(x, case["layout"])
+    _check_chain(case["id"], x, got, dets, case["dtype"])
 
 
-@pytest.mark.parametrize("mutant", lowp_band.BAND_MUTANTS)
-def test_band_mutants_are_rejected(mutant):
-    """The comparator rejects the model with a fault at the band's lower edge, on the same inputs as the kernels."""
-    x = _inputs(MUTANT_CASE)
-    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], x["biases"])
-    got = lm.lowp_chain(*args, mutant=mutant)
-    model, ref = lm.lowp_chain(*args), lm.oracle_chain(*args)
-    with pytest.raises(AssertionError):
-        lm.assert_chain_within_model(mutant, got, ref, model, MUTANT_CASE["dtype"], _absmax(x))
+@pytest.mark.parametrize("mutant,case_id", [(m, i) for m in lowp_band.BAND_MUTANTS for i in lowp_band.MUTANT_CASES[m]],
+                         ids=[f"{m}-{'bf16' if 'bf16' in i else 'fp16'}" for m in lowp_band.BAND_MUTANTS
+                              for i in lowp_band.MUTANT_CASES[m]])
+def test_band_mutants_are_rejected(mutant, case_id):
+    """The comparator rejects the model with a fault of the band, on the kernels' inputs and device."""
+    case = _BY_ID[case_id]
+    x = lowp_band.make_band_inputs(case, "cuda")
+    got = lm.lowp_chain(*_args(x), mutant=mutant)
+    model, ref = lm.lowp_chain(*_args(x)), lm.oracle_chain(*_args(x))
+    worst = dict(lm.WORST)  # the rejected runs stay out of the report of the kernels' worst ratios
+    try:
+        with pytest.raises(AssertionError):
+            lm.assert_chain_within_model(mutant, got, ref, model, case["dtype"], _absmax(x))
+    finally:
+        lm.WORST.clear()
+        lm.WORST.update(worst)
+
+
+# --------------------------------------------------------------------------- #
+# causal offsets at the ends of the C-ABI's int range
+# --------------------------------------------------------------------------- #
+# The C-ABI takes any int causal_offset (key j visible to row i iff j <= i + causal_offset); an offset >= Sk - 1 shows
+# every key and one <= -Sq none, so each chain must compute bitwise what it computes with Sk and -Sq in their place.
+I32_MAX, I32_MIN = 2 ** 31 - 1, -2 ** 31
+OFFSET_CASES = [
+    lowp_band.bcase(257, [(383, None, I32_MAX)], 128, BF16, tag="offmax_"),
+    lowp_band.bcase(257, [(383, -100, I32_MAX)], 64, FP16, tag="offmax_"),
+    lowp_band.bcase(200, [(257, -60, 40), (128, None, I32_MIN), (129, -300, 300)], 128, FP16, tag="offmin_"),
+    lowp_band.bcase(129, [(128, None, 0), (257, None, I32_MIN + 5), (64, -10, I32_MAX)], 64, BF16, tag="offmin_"),
+]
+
+
+def _in_range(masks, sq, sks):
+    """The masks with every causal offset clamped into [-Sq, Sk]."""
+    return [("band", lo, None if hi is None else min(max(hi, -sq), sk)) for (_, lo, hi), sk in zip(masks, sks)]
+
+
+@pytest.mark.parametrize("case", OFFSET_CASES, ids=[c["id"] for c in OFFSET_CASES])
+def test_causal_offset_at_int_range_ends(case):
+    x = lowp_band.make_band_inputs(case, "cuda")
+    y = dict(x, masks=_in_range(x["masks"], case["sq"], [k.shape[1] for k in x["ks"]]))
+    got, dets = native_chain(x)
+    want, want_dets = native_chain(y)
+    for name in ("o", "lse"):
+        assert torch.equal(got[name], want[name]), f"{name} differs from the chain with in-range offsets"
+    for c, (g, w) in enumerate(zip(got["states"], want["states"])):
+        assert torch.equal(g[0], w[0]) and torch.equal(g[1], w[1]), f"the state after chunk {c} differs"
+    (dq, dks, dvs), (wq, wks, wvs) = dets[0], want_dets[0]
+    assert torch.equal(dq, wq), "deterministic dQ differs from the chain with in-range offsets"
+    for c, (a, b, e, f) in enumerate(zip(dks, wks, dvs, wvs)):
+        assert torch.equal(a, b) and torch.equal(e, f), f"deterministic dK / dV of chunk {c} differ"
+    _check_chain(case["id"], x, got, dets, case["dtype"])
 
 
 # --------------------------------------------------------------------------- #
@@ -178,8 +221,8 @@ def test_flash_wrappers_window(monkeypatch, fn, causal, window, sq, sk, l2):
     left, right = window
     off = sk - sq
     band = ("band", None if left < 0 else off - left, 0 + off if causal else (None if right < 0 else off + right))
-    case = _case(sq, [(sk, band[1], band[2])], 128, BF16, H=4, tag=f"api_{fn}_{int(causal)}_{l2}_")
-    x = _inputs(case)
+    case = lowp_band.bcase(sq, [(sk, band[1], band[2])], 128, BF16, H=4, tag=f"api_{fn}_{int(causal)}_{l2}_")
+    x = lowp_band.make_band_inputs(case, "cuda")
     q, k, v = x["q"], x["ks"][0], x["vs"][0]
     if fn == "func":
         qq, kk, vv = (t.clone().requires_grad_() for t in (q, k, v))
@@ -236,3 +279,9 @@ def runs(tmp_path_factory):
 @pytest.mark.parametrize("job", RING_CASES, ids=lambda j: j["id"])
 def test_ring_window_within_model(runs, job):
     rb.check_window_case(job, rh.load_ring_case(job, runs.outdir(job["world"])))
+
+
+def test_report_worst_ratios():
+    """Runs last: prints the worst error / bound seen per output and dtype (the constants keep these <= 0.5)."""
+    for (name, dt), ((g, gcase), (r, rcase)) in sorted(lm.WORST.items()):
+        print(f"worst {name:>22s} {dt:>8s}: global {g:6.3f} ({gcase})  row {r:6.3f} ({rcase})")

@@ -239,6 +239,10 @@ def test_band_entry_points_reject_bad_masks_and_bands(nat):
         assert call(3, 0, 1) != 0 and b"lower_offset" in L.ba_last_error()  # lower edge above the upper one
         for mm, hi, lo in ((3, 5, -5), (2, 0, 7), (3, 0, 0), (1, 0, 0), (0, 0, 0)):
             assert call(mm, hi, lo) != 0 and b"null" in L.ba_last_error()  # valid: reaches the operand check
+        # causal offsets anywhere in the int range are valid; the band check compares the caller's values
+        for mm, hi, lo in ((1, 2 ** 31 - 1, 0), (1, -2 ** 31, 0), (3, 2 ** 31 - 1, 2 ** 31 - 1), (3, -2 ** 31, -2 ** 31)):
+            assert call(mm, hi, lo) != 0 and b"null" in L.ba_last_error()
+        assert call(3, -2 ** 31, -2 ** 31 + 1) != 0 and b"-2147483648" in L.ba_last_error()
     # the existing entry points keep rejecting the lower-edge bit
     rc = L.ba_fwd_chunk_gqa(z4, z4, z4, zr, z4, zr, z4, 1, 128, 128, 4, 2, 128, 1.0, 2, 0, 3, 1, None)
     assert rc != 0 and b"mask mode" in L.ba_last_error()
@@ -253,7 +257,8 @@ def test_band_symbols_bound(nat):
 
 
 def test_band_mutants_rejected_by_the_model_cpu():
-    """The 16-bit comparator rejects the faults of lowp_band.BAND_MUTANTS (model against model, on the CPU)."""
+    """The 16-bit comparator rejects the faults of lowp_band.BAND_MUTANTS this case reaches (model against model, on
+    the CPU); tests/test_lowp_band.py rejects every one of them on sweep cases of both dtypes."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import lowp_band
     import lowp_model as lm
@@ -265,7 +270,12 @@ def test_band_mutants_rejected_by_the_model_cpu():
     model, ref = lm.lowp_chain(*args), lm.oracle_chain(*args)
     absmax = [lm.scores_absmax(x["q"], x["ks"], x["scale"], x["masks"])]
     lm.assert_chain_within_model("band", model, ref, model, torch.bfloat16, absmax)
-    for mutant in lowp_band.BAND_MUTANTS:
+    vis = lowp_band.visible(257, 257, x["masks"][0])
+    live = [m for m in lowp_band.BAND_MUTANTS
+            if any(not torch.equal(lowp_band.vis_for(257, 257, x["masks"][0], None, m, side), vis)
+                   for side in ("fwd", "bwd"))]
+    assert {"band_lo_plus1_fwd", "band_lo_plus1_bwd", "band_i_end_short"} <= set(live), live
+    for mutant in live:
         with pytest.raises(AssertionError):
             lm.assert_chain_within_model(mutant, lm.lowp_chain(*args, mutant=mutant), ref, model, torch.bfloat16,
                                          absmax)
