@@ -113,11 +113,6 @@ def split2_gethalf(inp, first_dim, half_idx=0):
     return inp.narrow(dim, 0, n) if half_idx == 0 else inp.narrow(dim, n, inp.shape[dim] - n)
 
 
-def _half(t, dim, idx):
-    n = t.shape[dim] // 2
-    return t.narrow(dim, 0, n) if idx == 0 else t.narrow(dim, n, t.shape[dim] - n)
-
-
 def _nbytes(t) -> int:
     return t.numel() * t.element_size()
 
@@ -137,88 +132,15 @@ def _bias_kw(bias, c0=None, n=None):
     return {"bias": bias if c0 is None else bias.narrow(2, c0, n)}
 
 
-def _fwd_round(ops, q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, bias=None):
-    """One forward ring round, split over K/V blocks that fit L2 (each block is one kernel launch with
-    the carried state; the state pass costs 2 x 512 B per row and head, the block > 8 MB of math)."""
-    blk = _l2_block()
-    if k.shape[seq_dim] <= blk + blk // 2:
-        ops.fwd_chunk(q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, **_bias_kw(bias))
-        return
-    _fwd_blocks(ops, q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, blk, bias)
-
-
-def _fwd_blocks(ops, q, k, v, o_acc, lse, out, scale, causal, off, first, last, seq_dim, blk, bias=None,
-                before=None):
-    """A forward round as one launch per block of ``blk`` keys; ``before(c)``, if given, runs first in the step
-    of block c (host_stream.py waits there for the block's upload)."""
-    Sq, Sk = q.shape[seq_dim], k.shape[seq_dim]
-    n = (Sk + blk - 1) // blk
-    for c in range(n):
-        c0 = c * blk
-        kc, vc = k.narrow(seq_dim, c0, min(blk, Sk - c0)), v.narrow(seq_dim, c0, min(blk, Sk - c0))
-        if before is not None:
-            before(c)
-        if not causal:
-            ops.fwd_chunk(q, kc, vc, o_acc, lse, out, scale, False, 0, first and c == 0, last and c == n - 1, seq_dim,
-                          **_bias_kw(bias, c0, min(blk, Sk - c0)))
-            continue
-        # causal: rows before r_start see none of this block's keys (key c0+b visible to row a iff
-        # c0 + b <= a + off); keep r_start on a tile-pair boundary
-        r_start = max(0, (c0 - off) // 256 * 256)
-        if r_start >= Sq:
-            break
-        ops.fwd_chunk(q.narrow(seq_dim, r_start, Sq - r_start), kc, vc,
-                      o_acc.narrow(seq_dim, r_start, Sq - r_start), lse.narrow(2, r_start, Sq - r_start), None,
-                      scale, True, r_start + off - c0, first and c == 0, False, seq_dim,
-                      **_bias_kw(bias, c0, min(blk, Sk - c0)))
-    if causal and last:
-        ops.cast(o_acc, out, seq_dim)
-
-
-def _fwd_round_needs_state(k, seq_dim) -> bool:
-    blk = _l2_block()
-    return k.shape[seq_dim] > blk + blk // 2
-
-
-def _bwd_round(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
-               bias=None):
-    """One backward ring round, split over blocks of Q-bundle rows that fit L2."""
-    blk = _l2_block()
-    Sq = q.shape[seq_dim]
-    if Sq <= blk + blk // 2:
-        ops.bwd_chunk(g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
-                      **_bias_kw(bias))
-        return
-    for r0 in range(0, Sq, blk):
-        _bwd_rows(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
-                  r0, min(blk, Sq - r0), bias)
-
-
-def _bwd_rows(ops, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, causal, off, seq_dim, deterministic,
-              r0, n, bias=None):
-    """Rows [r0, r0+n) of a backward round as one launch over the keys they see (none: no launch)."""
-    kk, vv, dk, dv, o2, bkw = k, v, dk_acc, dv_acc, off, _bias_kw(bias)
-    if causal:
-        kmax = min(k.shape[seq_dim], r0 + n + off)  # keys visible to the last row of this block
-        if kmax <= 0:
-            return
-        kk, vv, bkw = k.narrow(seq_dim, 0, kmax), v.narrow(seq_dim, 0, kmax), _bias_kw(bias, 0, kmax)
-        dk, dv = dk_acc.narrow(seq_dim, 0, kmax), dv_acc.narrow(seq_dim, 0, kmax)
-        o2 = off + r0
-    ops.bwd_chunk(g.narrow(seq_dim, r0, n), q.narrow(seq_dim, r0, n), kk, vv, delta.narrow(2, r0, n),
-                  lse.narrow(2, r0, n), dq_part.narrow(seq_dim, r0, n), dk, dv, scale, causal, o2, seq_dim,
-                  deterministic, **bkw)
-
-
 # --------------------------------------------------------------------------- #
-# sliding-window (local) attention: band masks per round
+# launch planning: every call is a band of key positions around each query position
 # --------------------------------------------------------------------------- #
 def _check_window(window_size, causal):
-    """flash-attn's ``window_size=(left, right)`` (-1: that side unlimited; ``causal`` forces right = 0) ->
-    ``(left, right)`` with None for an unlimited side, or None when nothing is windowed: such a call runs exactly as
-    one without the argument."""
+    """flash-attn's ``window_size=(left, right)`` (-1 or None: unlimited; ``causal`` forces right = 0) -> the band
+    ``(left, right)`` of the call, None for an unlimited side: key position c is visible to query position a iff
+    a - left <= c <= a + right."""
     if window_size is None:
-        return None
+        window_size = (-1, -1)
     try:
         left, right = (int(x) for x in window_size)
     except (TypeError, ValueError):
@@ -226,11 +148,7 @@ def _check_window(window_size, causal):
     for name, x in (("left", left), ("right", right)):
         if x < -1:
             raise ValueError(f"window_size: {name} = {x}; it must be -1 (unlimited) or >= 0")
-    left = None if left == -1 else left
-    right = 0 if causal else (None if right == -1 else right)
-    if left is None and (right is None or causal):
-        return None
-    return left, right
+    return None if left == -1 else left, 0 if causal else (None if right == -1 else right)
 
 
 def _band(qn, kn, lo, hi):
@@ -247,72 +165,98 @@ def _band(qn, kn, lo, hi):
     return lo, hi
 
 
-def _round_pieces(layout, W, iq, jk, S, window):
-    """The pieces of the round that attends the Q shard of rank ``iq`` to the K/V shard of rank ``jk`` (``S`` rows
-    each): ``[(q0, qn, k0, kn, lo, hi)]``, rows and keys local to the shards, the band relative to the two views;
-    pieces whose band misses its view are left out.  ``window`` = (left, right) counts positions in the full
-    sequence: contiguous shards start at rank * S, zigzag shards are the halves rank and 2W-1-rank (one piece per
-    pair of halves), and striped token a of rank r sits at a W + r, so a + ceil((iq-jk-left)/W) <= c <=
-    a + floor((iq-jk+right)/W)."""
-    left, right = window
+def _sub(piece, r0, rn, c0, cn):
+    """Rows [r0, r0+rn) and keys [c0, c0+cn) of a piece (local to it) as a launch of their own, or None when none of
+    those rows sees any of those keys."""
+    qa, _, ka, _, lo, hi = piece
+    b = _band(rn, cn, None if lo is None else lo + r0 - c0, None if hi is None else hi + r0 - c0) \
+        if rn > 0 and cn > 0 else None
+    return None if b is None else (qa + r0, rn, ka + c0, cn) + b
+
+
+def _merged(pieces):
+    """A round's pieces as one launch over their bounding box when one band reproduces every sub-block exactly (so
+    zigzag's own round, and its j < i and j > i rounds, are one launch each), else as they are.  Each side of the box
+    band is taken from the first piece bounded on it: a side that binds in a piece is that piece's side exactly."""
+    if len(pieces) < 2:
+        return pieces
+    rows, keys = sorted({p[:2] for p in pieces}), sorted({p[2:4] for p in pieces})
+    q0, k0 = rows[0][0], keys[0][0]
+    qn, kn = sum(n for _, n in rows), sum(n for _, n in keys)
+    side = lambda s: next((p[s] - (p[0] - q0) + (p[2] - k0) for p in pieces if p[s] is not None), None)  # noqa: E731
+    box = (q0, qn, k0, kn, side(4), side(5))
+    have = {p[:4]: p for p in pieces}
+    if any(_sub(box, qa - q0, rn, ka - k0, cn) != have.get((qa, rn, ka, cn)) for qa, rn in rows for ka, cn in keys):
+        return pieces
+    return [_sub(box, 0, qn, 0, kn)]
+
+
+def _round_pieces(layout, W, iq, jk, Sq, Sk, band, merge=True):
+    """The pieces of the round that attends the Q shard of rank ``iq`` (``Sq`` rows) to the K/V shard of rank ``jk``
+    (``Sk`` keys): ``[(q0, qn, k0, kn, lo, hi)]``, rows and keys local to the shards, the band relative to the two
+    views; pieces whose band misses its view are left out, and with ``merge`` exact merges are made (``_merged``).
+    ``band`` = (left, right) counts positions in the full sequence: contiguous shards start at rank * S, zigzag shards
+    are the halves rank and 2W-1-rank (one piece per pair of halves), and striped token a of rank r sits at a W + r,
+    so a + ceil((iq-jk-left)/W) <= c <= a + floor((iq-jk+right)/W)."""
+    left, right = band
     if layout == "striped":
-        cand = [(0, S, 0, S, None if left is None else -((jk - iq + left) // W),
+        cand = [(0, Sq, 0, Sk, None if left is None else -((jk - iq + left) // W),
                  None if right is None else (iq - jk + right) // W)]
     else:
         if layout == "contiguous":
-            qs, ks = [(0, S, iq * S)], [(0, S, jk * S)]
+            qs, ks = [(0, Sq, iq * Sq)], [(0, Sk, jk * Sk)]
         else:
-            assert S % 2 == 0, "zigzag causal sharding needs an even local sequence length"
-            h = S // 2
+            assert Sq % 2 == 0 and Sk % 2 == 0, "zigzag causal sharding needs an even local sequence length"
+            h = Sq // 2
             qs = [(0, h, iq * h), (h, h, (2 * W - 1 - iq) * h)]
             ks = [(0, h, jk * h), (h, h, (2 * W - 1 - jk) * h)]
         cand = [(qa, qn, ka, kn, None if left is None else qg - kg - left, None if right is None else qg - kg + right)
                 for qa, qn, qg in qs for ka, kn, kg in ks]
-    out = []
-    for qa, qn, ka, kn, lo, hi in cand:
-        b = _band(qn, kn, lo, hi)
-        if b is not None:
-            out.append((qa, qn, ka, kn) + b)
-    return out
+    out = [p for p in (_sub(c, 0, c[1], 0, c[3]) for c in cand) if p is not None]
+    return _merged(out) if merge else out
+
+
+def _fwd_block(piece, c0, cn):
+    """Keys [c0, c0+cn) of a piece with only the rows that see them, the first row kept on a multiple of 256 (a
+    pair of 128-row tiles), or None."""
+    qn, lo, hi = piece[1], piece[4], piece[5]
+    r0 = 0 if hi is None else max(0, (c0 - hi) // 256 * 256)
+    r1 = qn if lo is None else min(qn, c0 + cn - lo)
+    return _sub(piece, r0, r1 - r0, c0, cn)
+
+
+def _bwd_block(piece, r0, rn):
+    """Rows [r0, r0+rn) of a piece with only the keys they see, or None."""
+    kn, lo, hi = piece[3], piece[4], piece[5]
+    c0 = 0 if lo is None else max(0, r0 + lo)
+    c1 = kn if hi is None else min(kn, r0 + rn + hi)
+    return _sub(piece, r0, rn, c0, c1 - c0)
 
 
 def _fwd_band_launches(pieces):
-    """Forward launches ``[(q0, qn, k0, kn, lo, hi)]`` of a round's pieces: a piece longer than the L2 block is split
-    over blocks of keys as in ``_fwd_blocks``, each launch taking only the rows that see its block."""
+    """Forward launches ``[(q0, qn, k0, kn, lo, hi)]`` of a round's pieces: a piece longer than 1.5 L2 blocks is
+    split over blocks of keys (each launch carries the state; the state pass costs 2 x 512 B per row and head, the
+    block > 8 MB of math)."""
     blk = _l2_block()
     out = []
-    for qa, qn, ka, kn, lo, hi in pieces:
-        if kn <= blk + blk // 2:
-            out.append((qa, qn, ka, kn, lo, hi))
-            continue
-        for c0 in range(0, kn, blk):
-            cn = min(blk, kn - c0)
-            r0 = 0 if hi is None else max(0, c0 - hi)
-            r1 = qn if lo is None else min(qn, c0 + cn - lo)
-            b = _band(r1 - r0, cn, None if lo is None else lo + r0 - c0, None if hi is None else hi + r0 - c0) \
-                if r0 < r1 else None
-            if b is not None:
-                out.append((qa + r0, r1 - r0, ka + c0, cn) + b)
+    for p in pieces:
+        if p[3] <= blk + blk // 2:
+            out.append(p)
+        else:
+            out += [x for x in (_fwd_block(p, c0, min(blk, p[3] - c0)) for c0 in range(0, p[3], blk)) if x]
     return out
 
 
 def _bwd_band_launches(pieces):
-    """Backward launches of a round's pieces: a piece with more rows than the L2 block is split over blocks of rows
-    as in ``_bwd_rows``, each launch taking only the keys its rows see."""
+    """Backward launches of a round's pieces: a piece with more than 1.5 L2 blocks of rows is split over blocks of
+    rows."""
     blk = _l2_block()
     out = []
-    for qa, qn, ka, kn, lo, hi in pieces:
-        if qn <= blk + blk // 2:
-            out.append((qa, qn, ka, kn, lo, hi))
-            continue
-        for r0 in range(0, qn, blk):
-            rn = min(blk, qn - r0)
-            c0 = 0 if lo is None else max(0, r0 + lo)
-            c1 = kn if hi is None else min(kn, r0 + rn + hi)
-            b = _band(rn, c1 - c0, None if lo is None else lo + r0 - c0, None if hi is None else hi + r0 - c0) \
-                if c0 < c1 else None
-            if b is not None:
-                out.append((qa + r0, rn, ka + c0, c1 - c0) + b)
+    for p in pieces:
+        if p[1] <= blk + blk // 2:
+            out.append(p)
+        else:
+            out += [x for x in (_bwd_block(p, r0, min(blk, p[1] - r0)) for r0 in range(0, p[1], blk)) if x]
     return out
 
 
@@ -366,14 +310,6 @@ def _alibi_kw(alibi, q0, k0):
     return {"alibi": (slopes, pos_q(q0) - pos_k(k0), pstride)}
 
 
-def _alibi_window(window, causal, alibi):
-    """A call with ALiBi runs the band launches (they know where their rows and keys sit), with the unwindowed band
-    when there is no window."""
-    if alibi is None or window is not None:
-        return window
-    return (None, 0 if causal else None)
-
-
 def _ring_alibi(slopes, layout, W, iq, jk, S):
     """The ALiBi of the round that attends the Q shard of rank iq to the K/V shard of rank jk (or None)."""
     if slopes is None:
@@ -384,19 +320,17 @@ def _ring_alibi(slopes, layout, W, iq, jk, S):
 
 
 class _BandForward:
-    """The launches of a windowed forward, known up front for every round, and their first / last duties.  Skipped
-    launches must not drop either: the state is started by the first launch only if it covers every row (otherwise
-    it starts as O = 0, lse = -inf in memory), and the output is written by the last launch only if it covers every
-    row (otherwise it is cast from the fp32 state at the end)."""
+    """The forward launches of a call, known up front for every round, and their first / last duties.  The state is
+    started by the first launch only if it covers every row (otherwise it starts as O = 0, lse = -inf in memory); the
+    last launch writes its own rows in 16 bit, and ``finish`` casts the other rows from the fp32 state."""
 
     def __init__(self, rounds, q, lse, S):
         flat = [x for launches in rounds for x in launches]
-        full = lambda x: x[0] == 0 and x[1] == S  # noqa: E731
-        self.first = bool(flat) and full(flat[0])
-        self.last = bool(flat) and full(flat[-1])
+        self.first = bool(flat) and flat[0][0] == 0 and flat[0][1] == S
+        self.last_rows = flat[-1][:2] if flat else (0, 0)
         self.n, self.done = len(flat), 0
         self.o_acc = None
-        if not (self.n == 1 and self.first and self.last):
+        if not (self.n == 1 and self.first):
             self.o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device)
         if not self.first:
             self.o_acc.zero_()
@@ -405,7 +339,7 @@ class _BandForward:
     def run(self, ops, launches, q, k, v, lse, out, scale, seq_dim, bias=None, alibi=None):
         for q0, qn, k0, kn, lo, hi in launches:
             first = self.first and self.done == 0
-            last = self.last and self.done == self.n - 1
+            last = self.done == self.n - 1
             rows = lambda t: t.narrow(seq_dim, q0, qn)  # noqa: E731
             ops.fwd_chunk(rows(q), k.narrow(seq_dim, k0, kn), v.narrow(seq_dim, k0, kn),
                           None if self.o_acc is None else rows(self.o_acc), lse.narrow(2, q0, qn),
@@ -414,8 +348,10 @@ class _BandForward:
             self.done += 1
 
     def finish(self, ops, out, seq_dim):
-        if not self.last:
-            ops.cast(self.o_acc, out, seq_dim)
+        q0, qn = self.last_rows
+        for r0, rn in ((0, q0), (q0 + qn, out.shape[seq_dim] - q0 - qn)):
+            if rn > 0:
+                ops.cast(self.o_acc.narrow(seq_dim, r0, rn), out.narrow(seq_dim, r0, rn), seq_dim)
 
 
 def _bwd_band_run(ops, launches, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic,
@@ -437,35 +373,15 @@ def _check_inputs(q, k, v, seq_dim):
     assert q.dtype == k.dtype == v.dtype, "q, k, v must share a dtype"
 
 
-def _fwd_dispatch(ops, mode, r, W, i, j, q, cur_k, cur_v, o_acc, lse, out, scale, seq_dim):
-    """The kernel work of forward round r on rank i holding the K/V shard of rank j (SURVEY.md App. B)."""
-    first, last = r == 1, r == W
-    if mode == "none":
-        _fwd_round(ops, q, cur_k, cur_v, o_acc, lse, out, scale, False, 0, first, last, seq_dim)
-    elif mode == "zigzag":
-        if r == 1:  # own shard: plain causal (:221-224)
-            _fwd_round(ops, q, cur_k, cur_v, o_acc, lse, out, scale, True, 0, first, last, seq_dim)
-        elif j < i:  # split_kv: all Q x first half of K/V (:225-231)
-            _fwd_round(ops, q, _half(cur_k, seq_dim, 0), _half(cur_v, seq_dim, 0), o_acc, lse, out, scale,
-                       False, 0, False, last, seq_dim)
-        else:  # second half of Q x all K/V, merged into the second half of the state (:232-235)
-            _fwd_round(ops, _half(q, seq_dim, 1), cur_k, cur_v, _half(o_acc, seq_dim, 1), _half(lse, 2, 1),
-                       _half(out, seq_dim, 1), scale, False, 0, False, last, seq_dim)
-            if last:  # rows the last round did not visit: hand their finished state over
-                ops.cast(_half(o_acc, seq_dim, 0), _half(out, seq_dim, 0), seq_dim)
-    elif mode == "striped":
-        # source rank ahead of us -> strictly-lower-triangular (causal_shift, :454,:463-475)
-        _fwd_round(ops, q, cur_k, cur_v, o_acc, lse, out, scale, True, -1 if j > i else 0, first, last, seq_dim)
-    else:
-        raise ValueError(mode)
-
-
 # --------------------------------------------------------------------------- #
 # forward ring (reference OpBurstAttn.forward :171-253, OpBurstAttnStrip.forward :411-493)
 # --------------------------------------------------------------------------- #
-def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None, alibi=None):
-    """mode: "none" (non-causal) | "zigzag" | "striped".  Returns (out, lse[B,H,S] fp32).  With a ``window``
-    (``_check_window``) the rounds run the band launches of ``_round_pieces`` for the shard ``layout`` instead.
+def _ring_forward(q, k, v, scale, seq_dim, layout, band, topo, alibi=None):
+    """layout: the shards ("contiguous" | "zigzag" | "striped"); band: the call's (left, right) from
+    ``_check_window``.  Returns (out, lse[B,H,S] fp32).  Each round runs the launches of ``_round_pieces``: the
+    reference's zigzag rounds (plain causal own shard :221-224, all Q x first half of K/V :225-231, second half of Q x
+    all K/V :232-235) and striped rounds (strictly lower triangular from a source rank ahead, :454,:463-475) are the
+    pieces of the causal band.
 
     Rounds run in M cycles of L steps (the flat ring is one cycle, L = W).  Within a cycle K/V hop round the
     intra-node ring; on the hierarchical ring (reference comm.py:187-254, SURVEY.md Appendix C) the block a
@@ -474,25 +390,17 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None,
     send-side copy is made: the cycle's starting block is never a receive target while it is in flight (two
     inter-node buffers alternate).
 
-    ``alibi`` (fp32 slopes [B, H] from ``_check_alibi``) runs the band launches too, with the unwindowed band when
-    there is no window, so that every launch knows where its rows and keys sit in the full sequence."""
+    ``alibi`` (fp32 slopes [B, H] from ``_check_alibi``) gives every launch where its rows and keys sit in the full
+    sequence; its pieces are not merged, since zigzag positions are not affine across the two halves."""
     ops = get_ops()
-    window = _alibi_window(window, mode != "none", alibi)
     ring, inter, _ = topo.rings()
     L, M, W, i = topo.L, topo.M, topo.W, topo.rank
     B, S, H = q.shape[0], q.shape[seq_dim], q.shape[3 - seq_dim]
-    if mode == "zigzag":
-        assert S % 2 == 0, "zigzag causal sharding needs an even local sequence length"
     out = torch.empty_like(q)
     lse = torch.empty((B, H, S), dtype=torch.float32, device=q.device)
-    band = None
-    if window is not None:
-        band = _BandForward([_fwd_band_launches(_round_pieces(layout, W, i, topo.source(r), S, window))
-                             for r in range(1, W + 1)], q, lse, S)
-        o_acc = None
-    else:
-        need_state = W > 1 or _fwd_round_needs_state(k, seq_dim)
-        o_acc = torch.empty(q.shape, dtype=torch.float32, device=q.device) if need_state else None
+    plan = [_fwd_band_launches(_round_pieces(layout, W, i, topo.source(r), S, k.shape[seq_dim], band, alibi is None))
+            for r in range(1, W + 1)]
+    state = _BandForward(plan, q, lse, S)
     if W > 1:
         k, v = k.contiguous(), v.contiguous()
     ring.begin(q, [_nbytes(k), _nbytes(v)] * min(2, L - 1))
@@ -508,52 +416,25 @@ def _ring_forward(q, k, v, scale, seq_dim, mode, topo, window=None, layout=None,
             if t != L - 1:
                 nxt = recv[(r - 1) % len(recv)]
                 ring.post(cur, nxt)
-            if band is None:
-                _fwd_dispatch(ops, mode, r, W, i, j, q, cur[0], cur[1], o_acc, lse, out, scale, seq_dim)
-            else:  # a round whose shard lies outside every row's window launches nothing
-                band.run(ops, _fwd_band_launches(_round_pieces(layout, W, i, j, S, window)), q, cur[0], cur[1], lse,
-                         out, scale, seq_dim, alibi=_ring_alibi(alibi, layout, W, i, j, S))
+            # a round whose shard lies outside every row's band launches nothing
+            state.run(ops, plan[r - 1], q, cur[0], cur[1], lse, out, scale, seq_dim,
+                      alibi=_ring_alibi(alibi, layout, W, i, j, S))
             if t != L - 1:
                 ring.wait()
                 cur = nxt
             elif c != M - 1:
                 inter.wait()
                 cur = xbuf[c % len(xbuf)]
-    if band is not None:
-        band.finish(ops, out, seq_dim)
+    state.finish(ops, out, seq_dim)
     return out, lse
 
 
 # --------------------------------------------------------------------------- #
 # backward ring (reference OpBurstAttn.backward :256-398, OpBurstAttnStrip.backward :496-613)
 # --------------------------------------------------------------------------- #
-def _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, scale, seq_dim, deterministic):
-    """The kernel work of backward round r: K/V at home on rank i, Q-bundle of rank j (SURVEY.md App. B)."""
-    dlt, g, qq, ls = bundle
-    if mode == "none":
-        _bwd_round(ops, g, qq, k, v, dlt, ls, dq_part, dk_acc, dv_acc, scale, False, 0, seq_dim, deterministic)
-    elif mode == "zigzag":
-        if r == 1:
-            _bwd_round(ops, g, qq, k, v, dlt, ls, dq_part, dk_acc, dv_acc, scale, True, 0, seq_dim, deterministic)
-        elif j < i:  # split_q: second half of the bundle x all K/V (:322-345,:383-386)
-            _bwd_round(ops, _half(g, seq_dim, 1), _half(qq, seq_dim, 1), k, v, _half(dlt, 2, 1), _half(ls, 2, 1),
-                       _half(dq_part, seq_dim, 1), dk_acc, dv_acc, scale, False, 0, seq_dim, deterministic)
-        else:  # whole bundle x first half of K/V (:347-367,:387-390)
-            _bwd_round(ops, g, qq, _half(k, seq_dim, 0), _half(v, seq_dim, 0), dlt, ls, dq_part,
-                       _half(dk_acc, seq_dim, 0), _half(dv_acc, seq_dim, 0), scale, False, 0, seq_dim,
-                       deterministic)
-    elif mode == "striped":
-        # K/V home on i, bundle from j: strict iff j < i (causal_shift, :529)
-        _bwd_round(ops, g, qq, k, v, dlt, ls, dq_part, dk_acc, dv_acc, scale, True, -1 if j < i else 0, seq_dim,
-                   deterministic)
-    else:
-        raise ValueError(mode)
-
-
-def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, deterministic, window=None, layout=None,
-                   alibi=None):
+def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, layout, band, topo, deterministic, alibi=None):
+    """Backward of ``_ring_forward``: round r attends the Q-bundle of rank j = source(r) to the K/V at home."""
     ops = get_ops()
-    window = _alibi_window(window, mode != "none", alibi)
     W, i = topo.W, topo.rank
     dev = q.device
     q, k, v, d_o, out = (t.contiguous() for t in (q, k, v, d_o, out))
@@ -569,13 +450,10 @@ def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, mode, topo, determini
     dv_acc = torch.zeros(v.shape, **f32)
 
     def round_kernel(r, j, bundle, dq_part):
-        if window is None:
-            _bwd_dispatch(ops, mode, r, i, j, bundle, dq_part, k, v, dk_acc, dv_acc, scale, seq_dim, deterministic)
-            return
         dlt, g, qq, ls = bundle  # the bundle of rank j against the K/V at home: rows of j, keys of i
-        _bwd_band_run(ops, _bwd_band_launches(_round_pieces(layout, W, j, i, S, window)), g, qq, k, v, dlt, ls,
-                      dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic,
-                      alibi=_ring_alibi(alibi, layout, W, j, i, S))
+        pieces = _round_pieces(layout, W, j, i, S, k.shape[seq_dim], band, alibi is None)
+        _bwd_band_run(ops, _bwd_band_launches(pieces), g, qq, k, v, dlt, ls, dq_part, dk_acc, dv_acc, scale, seq_dim,
+                      deterministic, alibi=_ring_alibi(alibi, layout, W, j, i, S))
 
     bundle = [delta, d_o, q, lse.contiguous()]
     if W == 1:
@@ -691,7 +569,7 @@ def _bwd_rounds(ops, topo, round_kernel, bundle, q, seq_dim):
 def _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
              double_group, window_size=(-1, -1), alibi_slopes=None):
     assert not causal or flash == "cuda", "Causal attention only supported for Flash v2"
-    ctx.window = _check_window(window_size, causal)
+    ctx.band = _check_window(window_size, causal)
     ctx.alibi = _check_alibi(alibi_slopes, q, 2 if flash in ["cuda", "triton"] else 1)
     ctx.softmax_scale = 1 / math.sqrt(q.shape[-1]) if softmax_scale is None else softmax_scale
     ctx.flash = None if flash not in ["cuda", "triton"] else flash
@@ -724,12 +602,11 @@ def _unpad(t, D):
     return t if t.shape[-1] == D else t[..., :D].contiguous()
 
 
-def _op_forward(ctx, q, k, v, mode, layout):
-    """mode: the schedule of the call without a window; layout: its shards ("contiguous" | "zigzag" | "striped"),
-    which a window needs even where the mask-free schedule does not."""
-    ctx.host = False
+def _op_forward(ctx, q, k, v, layout):
+    """layout: the call's shards ("contiguous" | "zigzag" | "striped")."""
+    ctx.host, ctx.layout = False, layout
     if q.device.type == "cpu" and getattr(get_ops(), "name", "") == "sm90":  # (tests inject CPU chunk operators)
-        if ctx.window is not None:
+        if ctx.band != _check_window(None, ctx.causal):
             raise NotImplementedError("window_size is not supported with host-resident (pinned CPU) operands; pass "
                                       "CUDA tensors")
         if ctx.alibi is not None:
@@ -742,13 +619,12 @@ def _op_forward(ctx, q, k, v, mode, layout):
                             "no CPU implementation")
         assert ctx.topo.W == 1, "host-resident operands are supported on a single rank only (pass device tensors)"
         assert q.shape[-1] in getattr(get_ops(), "tile_head_dims", (q.shape[-1],)), "host-resident operands need head_dim 64 or 128"
-        ctx.host, ctx.mode, ctx.head_dim = True, mode, q.shape[-1]
-        o_host, saved = host_stream.forward(q, k, v, ctx.softmax_scale, ctx.seq_dim, mode != "none", _l2_block())
+        ctx.host, ctx.head_dim = True, q.shape[-1]
+        o_host, saved = host_stream.forward(q, k, v, ctx.softmax_scale, ctx.seq_dim, ctx.band, _l2_block())
         ctx.save_for_backward(*saved)
         return o_host
     (qp, kp, vp), ctx.head_dim = _pad_head_dim(get_ops(), [q, k, v])
-    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, mode, ctx.topo, ctx.window, layout, ctx.alibi)
-    ctx.mode, ctx.layout = mode, layout
+    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, layout, ctx.band, ctx.topo, ctx.alibi)
     ctx.save_for_backward(qp, kp, vp, lse, out)
     return _unpad(out, ctx.head_dim)
 
@@ -756,13 +632,13 @@ def _op_forward(ctx, q, k, v, mode, layout):
 def _op_backward(ctx, grad_output):
     if ctx.host:
         from . import host_stream
-        grads = host_stream.backward(grad_output, ctx.saved_tensors, ctx.softmax_scale, ctx.seq_dim,
-                                     ctx.mode != "none", _l2_block(), ctx.deterministic)
+        grads = host_stream.backward(grad_output, ctx.saved_tensors, ctx.softmax_scale, ctx.seq_dim, ctx.band,
+                                     _l2_block(), ctx.deterministic)
         return tuple(grads) + (None,) * 9
     q, k, v, lse, out = ctx.saved_tensors
     (g,), _ = _pad_head_dim(get_ops(), [grad_output])
-    dq, dk, dv = _ring_backward(g, q, k, v, out, lse, ctx.softmax_scale, ctx.seq_dim, ctx.mode, ctx.topo,
-                                ctx.deterministic, ctx.window, ctx.layout, ctx.alibi)
+    dq, dk, dv = _ring_backward(g, q, k, v, out, lse, ctx.softmax_scale, ctx.seq_dim, ctx.layout, ctx.band, ctx.topo,
+                                ctx.deterministic, ctx.alibi)
     return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 9
 
 
@@ -782,7 +658,7 @@ class OpBurstAttn(torch.autograd.Function):
                 alibi_slopes=None):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
                  double_group, window_size, alibi_slopes)
-        return _op_forward(ctx, q, k, v, "zigzag" if causal else "none", "zigzag" if causal else "contiguous")
+        return _op_forward(ctx, q, k, v, "zigzag" if causal else "contiguous")
 
     @staticmethod
     def backward(ctx, grad_output):
@@ -799,7 +675,7 @@ class OpBurstAttnStrip(torch.autograd.Function):
                 alibi_slopes=None):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
                  double_group, window_size, alibi_slopes)
-        return _op_forward(ctx, q, k, v, "striped" if causal else "none", "striped")
+        return _op_forward(ctx, q, k, v, "striped")
 
     @staticmethod
     def backward(ctx, grad_output):

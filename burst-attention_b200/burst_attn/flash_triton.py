@@ -33,9 +33,8 @@ import math
 
 import torch
 
-from .burst_attn_interface import (_alibi_window, _band, _BandForward, _bwd_band_launches, _bwd_band_run,
-                                   _bwd_round, _check_alibi, _check_window, _fwd_band_launches, _fwd_round,
-                                   _fwd_round_needs_state, _pad_head_dim, _positions, _unpad)
+from .burst_attn_interface import (_band, _BandForward, _bwd_band_launches, _bwd_band_run, _check_alibi,
+                                   _check_window, _fwd_band_launches, _pad_head_dim, _positions, _unpad)
 from .chunk_ops import get_ops
 
 __all__ = ["flash_attn_func", "flash_attn_kvpacked_func", "flash_attn_qkvpacked_func"]
@@ -53,9 +52,9 @@ def _key_bias(bias, q, k):
     return b3.expand(B, H, Sk)
 
 
-def _window_pieces(window, Sq, Sk):
-    """The one piece (``_round_pieces`` form) of a windowed local call, or none when no row sees a key."""
-    left, right = window
+def _local_pieces(band, Sq, Sk):
+    """The one piece (``_round_pieces`` form) of a local call, bottom-right aligned, or none when no row sees a key."""
+    left, right = band
     off = Sk - Sq
     b = _band(Sq, Sk, None if left is None else off - left, None if right is None else off + right)
     return [] if b is None else [(0, Sq, 0, Sk) + b]
@@ -70,26 +69,21 @@ def _local_alibi(slopes, Sq, Sk):
     return slopes, pos_q, pos_k, 1
 
 
-def _local_forward(q, k, v, causal, softmax_scale, bias=None, window=None, alibi=None):
+def _local_forward(q, k, v, softmax_scale, bias, band, alibi):
     ops = get_ops()
     scale = softmax_scale or 1.0 / math.sqrt(q.shape[-1])
     (qp, kp, vp), D = _pad_head_dim(ops, [q, k, v])
     B, Sq, H = qp.shape[0], qp.shape[1], qp.shape[2]
     out = torch.empty(qp.shape, dtype=qp.dtype, device=qp.device)
     lse = torch.empty((B, H, Sq), dtype=torch.float32, device=qp.device)
-    window = _alibi_window(window, causal, alibi)
-    if window is not None:
-        launches = _fwd_band_launches(_window_pieces(window, Sq, kp.shape[1]))
-        band = _BandForward([launches], qp, lse, Sq)
-        band.run(ops, launches, qp, kp, vp, lse, out, scale, 1, bias, _local_alibi(alibi, Sq, kp.shape[1]))
-        band.finish(ops, out, 1)
-        return out, lse, scale, (qp, kp, vp), D
-    o_acc = torch.empty(qp.shape, dtype=torch.float32, device=qp.device) if _fwd_round_needs_state(kp, 1) else None
-    _fwd_round(ops, qp, kp, vp, o_acc, lse, out, scale, causal, kp.shape[1] - Sq, True, True, 1, bias)
+    launches = _fwd_band_launches(_local_pieces(band, Sq, kp.shape[1]))
+    state = _BandForward([launches], qp, lse, Sq)
+    state.run(ops, launches, qp, kp, vp, lse, out, scale, 1, bias, _local_alibi(alibi, Sq, kp.shape[1]))
+    state.finish(ops, out, 1)
     return out, lse, scale, (qp, kp, vp), D
 
 
-def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, deterministic=False, window=None, alibi=None):
+def _local_backward(do, qp, kp, vp, out, lse, scale, bias, band, alibi, deterministic=False):
     ops = get_ops()
     (g,), _ = _pad_head_dim(ops, [do])
     g, out = g.contiguous(), out.contiguous()
@@ -98,12 +92,8 @@ def _local_backward(do, qp, kp, vp, out, lse, causal, scale, bias=None, determin
     ops.delta(out, g, delta, 1)
     f32 = dict(dtype=torch.float32, device=qp.device)
     dq, dk, dv = torch.zeros(qp.shape, **f32), torch.zeros(kp.shape, **f32), torch.zeros(vp.shape, **f32)
-    window = _alibi_window(window, causal, alibi)
-    if window is not None:
-        _bwd_band_run(ops, _bwd_band_launches(_window_pieces(window, Sq, kp.shape[1])), g, qp, kp, vp, delta, lse, dq,
-                      dk, dv, scale, 1, deterministic, bias, _local_alibi(alibi, Sq, kp.shape[1]))
-        return dq, dk, dv
-    _bwd_round(ops, g, qp, kp, vp, delta, lse, dq, dk, dv, scale, causal, kp.shape[1] - Sq, 1, deterministic, bias)
+    _bwd_band_run(ops, _bwd_band_launches(_local_pieces(band, Sq, kp.shape[1])), g, qp, kp, vp, delta, lse, dq, dk, dv,
+                  scale, 1, deterministic, bias, _local_alibi(alibi, Sq, kp.shape[1]))
     return dq, dk, dv
 
 
@@ -139,19 +129,17 @@ class FlashAttnFunc(torch.autograd.Function):
         _check(bias, q, k, v)
         _check_heads(q, k)
         ctx.bias = _key_bias(bias, q, k)
-        ctx.window = _check_window(window_size, causal)
+        ctx.band = _check_window(window_size, causal)
         ctx.alibi = _alibi(alibi_slopes, bias, q)
-        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, k, v, causal, softmax_scale, ctx.bias,
-                                                                          ctx.window, ctx.alibi)
+        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, k, v, softmax_scale, ctx.bias, ctx.band,
+                                                                          ctx.alibi)
         ctx.save_for_backward(*saved, out, lse)
-        ctx.causal = causal
         return _unpad(out, ctx.head_dim)
 
     @staticmethod
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
-        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
-                                     window=ctx.window, alibi=ctx.alibi)
+        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.softmax_scale, ctx.bias, ctx.band, ctx.alibi)
         return (_cast(dq, qp, ctx.head_dim), _cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim), None, None, None,
                 None, None)
 
@@ -165,19 +153,17 @@ class FlashAttnKVPackedFunc(torch.autograd.Function):
         _check(bias, q, kv)
         _check_heads(q, kv[:, :, 0])
         ctx.bias = _key_bias(bias, q, kv[:, :, 0])
-        ctx.window = _check_window(window_size, causal)
+        ctx.band = _check_window(window_size, causal)
         ctx.alibi = _alibi(alibi_slopes, bias, q)
-        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, kv[:, :, 0], kv[:, :, 1], causal,
-                                                                          softmax_scale, ctx.bias, ctx.window, ctx.alibi)
+        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(q, kv[:, :, 0], kv[:, :, 1],
+                                                                          softmax_scale, ctx.bias, ctx.band, ctx.alibi)
         ctx.save_for_backward(*saved, out, lse)
-        ctx.causal = causal
         return _unpad(out, ctx.head_dim)
 
     @staticmethod
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
-        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
-                                     window=ctx.window, alibi=ctx.alibi)
+        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.softmax_scale, ctx.bias, ctx.band, ctx.alibi)
         dkv = torch.stack([_cast(dk, kp, ctx.head_dim), _cast(dv, vp, ctx.head_dim)], dim=2)
         return _cast(dq, qp, ctx.head_dim), dkv, None, None, None, None, None
 
@@ -189,19 +175,17 @@ class FlashAttnQKVPackedFunc(torch.autograd.Function):
     def forward(ctx, qkv, bias=None, causal=False, softmax_scale=None, window_size=(-1, -1), alibi_slopes=None):
         _check(bias, qkv)
         ctx.bias = _key_bias(bias, qkv[:, :, 0], qkv[:, :, 1])
-        ctx.window = _check_window(window_size, causal)
+        ctx.band = _check_window(window_size, causal)
         ctx.alibi = _alibi(alibi_slopes, bias, qkv[:, :, 0])
-        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], causal,
-                                                                          softmax_scale, ctx.bias, ctx.window, ctx.alibi)
+        out, lse, ctx.softmax_scale, saved, ctx.head_dim = _local_forward(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2],
+                                                                          softmax_scale, ctx.bias, ctx.band, ctx.alibi)
         ctx.save_for_backward(*saved, out, lse)
-        ctx.causal = causal
         return _unpad(out, ctx.head_dim)
 
     @staticmethod
     def backward(ctx, do):
         qp, kp, vp, out, lse = ctx.saved_tensors
-        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.causal, ctx.softmax_scale, ctx.bias,
-                                     window=ctx.window, alibi=ctx.alibi)
+        dq, dk, dv = _local_backward(do, qp, kp, vp, out, lse, ctx.softmax_scale, ctx.bias, ctx.band, ctx.alibi)
         dqkv = torch.stack([_cast(t, qp, ctx.head_dim) for t in (dq, dk, dv)], dim=2)
         return dqkv, None, None, None, None, None
 

@@ -1,10 +1,11 @@
 """Host-resident operands (single rank): ``burst_attn_func`` called with CPU tensors in pinned memory.
 
-The L2-blocked drivers (burst_attn_interface.py ``_fwd_round`` / ``_bwd_round``) consume K/V block by block in the
-forward and finish dQ row block by row block in the backward, so when Q/K/V/dO live in HOST memory the copies can
-ride under the kernels instead of bracketing the call:
+The launch planner (burst_attn_interface.py) splits a call over L2 blocks: K/V block by block in the forward
+(``_fwd_block``) and dQ row block by row block in the backward (``_bwd_block``), so when Q/K/V/dO live in HOST memory
+the copies can ride under the kernels instead of bracketing the call:
 
   forward   up   : Q, then K/V block c on the upload stream (event per block); the kernel of block c waits for it
+                   (the forward always splits at the block; first / last duties as in ``_BandForward``)
             down : O after the last block -- under the backward, if one follows
   backward  up   : dO row block r (event per block); delta and the backward kernel of block r wait for it
             down : dQ row block r as soon as its sub-launch has finished; the LAST row block is launched per key
@@ -21,7 +22,7 @@ from __future__ import annotations
 
 import torch
 
-from .burst_attn_interface import _bwd_rows, _fwd_blocks
+from .burst_attn_interface import _BandForward, _bwd_band_run, _bwd_block, _fwd_block, _round_pieces, _sub
 from .chunk_ops import get_ops
 
 _streams = {}
@@ -46,8 +47,9 @@ def is_host_call(q, k, v) -> bool:
     return q.device.type == "cpu" and k.device.type == "cpu" and v.device.type == "cpu" and torch.cuda.is_available()
 
 
-def forward(q, k, v, scale, seq_dim, causal, blk):
-    """q, k, v: pinned CPU [B,S,H,D] (seq_dim 1) or [B,H,S,D] (seq_dim 2).  Returns (o_host, saved device tensors)."""
+def forward(q, k, v, scale, seq_dim, band, blk):
+    """q, k, v: pinned CPU [B,S,H,D] (seq_dim 1) or [B,H,S,D] (seq_dim 2); band: the call's (left, right) without a
+    window.  Returns (o_host, saved device tensors)."""
     ops = get_ops()
     dev = torch.device("cuda", torch.cuda.current_device())
     cur = torch.cuda.current_stream(dev)
@@ -60,8 +62,9 @@ def forward(q, k, v, scale, seq_dim, causal, blk):
     out = torch.empty_like(qd)
     lse = torch.empty((B, H, S), dtype=torch.float32, device=dev)
     kblocks = _blocks(Sk, blk)
-    n = len(kblocks)
-    o_acc = torch.empty(qd.shape, dtype=torch.float32, device=dev) if (n > 1 or causal) else None
+    piece, = _round_pieces("contiguous", 1, 0, 0, S, Sk, band)
+    launches = [x for x in (_fwd_block(piece, c0, cn) for c0, cn in kblocks) if x]
+    state = _BandForward([launches], qd, lse, S)
     up.wait_stream(cur)  # the fresh device buffers may reuse memory the compute stream is still working on
     ev = []
     with torch.cuda.stream(up):
@@ -74,8 +77,10 @@ def forward(q, k, v, scale, seq_dim, causal, blk):
             ev.append(e)
     for t in (qd, kd, vd):
         t.record_stream(up)
-    _fwd_blocks(ops, qd, kd, vd, o_acc, lse, out, scale, causal, 0, True, True, seq_dim, blk,
-                before=lambda c: cur.wait_event(ev[c]))
+    for x in launches:
+        cur.wait_event(ev[(x[2] + x[3] - 1) // blk])  # the last K/V block the launch reads
+        state.run(ops, [x], qd, kd, vd, lse, out, scale, seq_dim)
+    state.finish(ops, out, seq_dim)
     o_host = _pinned_like(q.shape, q.dtype)
     done = torch.cuda.Event()
     done.record(cur)
@@ -86,7 +91,7 @@ def forward(q, k, v, scale, seq_dim, causal, blk):
     return o_host, (qd, kd, vd, out, lse)
 
 
-def backward(d_o, saved, scale, seq_dim, causal, blk, deterministic):
+def backward(d_o, saved, scale, seq_dim, band, blk, deterministic):
     """d_o: pinned CPU gradient of O.  Returns pinned CPU (dq, dk, dv)."""
     ops = get_ops()
     qd, kd, vd, out, lse = saved
@@ -105,6 +110,7 @@ def backward(d_o, saved, scale, seq_dim, causal, blk, deterministic):
     dq16, dk16, dv16 = torch.empty_like(qd), torch.empty_like(kd), torch.empty_like(vd)
     dq_h, dk_h, dv_h = (_pinned_like(t.shape, t.dtype) for t in (qd, kd, vd))
     rblocks, kblocks = _blocks(S, blk), _blocks(Sk, blk)
+    piece, = _round_pieces("contiguous", 1, 0, 0, S, Sk, band)
     up.wait_stream(cur)
     ev = []
     with torch.cuda.stream(up):
@@ -125,23 +131,21 @@ def backward(d_o, saved, scale, seq_dim, causal, blk, deterministic):
             down.wait_event(e)
             host.narrow(seq_dim, s0, sn).copy_(lowp.narrow(seq_dim, s0, sn), non_blocking=True)
 
+    def run(launch):
+        if launch is not None:
+            _bwd_band_run(ops, [launch], g, qd, kd, vd, delta, lse, dq_acc, dk_acc, dv_acc, scale, seq_dim,
+                          deterministic)
+
     for i, (r0, rn) in enumerate(rblocks):
         cur.wait_event(ev[i])
-        gb, qb = g.narrow(seq_dim, r0, rn), qd.narrow(seq_dim, r0, rn)
-        db, lb = delta.narrow(2, r0, rn), lse.narrow(2, r0, rn)
-        ops.delta(out.narrow(seq_dim, r0, rn), gb, db, seq_dim)
-        dqb = dq_acc.narrow(seq_dim, r0, rn)
+        ops.delta(out.narrow(seq_dim, r0, rn), g.narrow(seq_dim, r0, rn), delta.narrow(2, r0, rn), seq_dim)
         if i < len(rblocks) - 1:
-            _bwd_rows(ops, g, qd, kd, vd, delta, lse, dq_acc, dk_acc, dv_acc, scale, causal, 0, seq_dim, deterministic,
-                      r0, rn)
+            run(_bwd_block(piece, r0, rn))
             ship(dq_acc, dq16, dq_h, r0, rn)
             continue
         # last row block: one launch per key block, so every dK / dV block is final right after its launch
         for k0, kn in kblocks:
-            if not causal or k0 <= r0 + rn - 1:
-                ops.bwd_chunk(gb, qb, kd.narrow(seq_dim, k0, kn), vd.narrow(seq_dim, k0, kn), db, lb, dqb,
-                              dk_acc.narrow(seq_dim, k0, kn), dv_acc.narrow(seq_dim, k0, kn), scale, causal,
-                              r0 - k0, seq_dim, deterministic)
+            run(_sub(piece, r0, rn, k0, kn))
             ship(dk_acc, dk16, dk_h, k0, kn)
             ship(dv_acc, dv16, dv_h, k0, kn)
         ship(dq_acc, dq16, dq_h, r0, rn)

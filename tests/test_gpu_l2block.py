@@ -1,6 +1,6 @@
 """The code path the headline bench runs at N=1/2/4: every ring round goes through the L2-blocked
-sub-launch drivers ``_fwd_round`` / ``_bwd_round`` (burst_attn_interface.py) -- K/V blocks with
-carried state forward, Q-row blocks backward, causal views with r_start / kmax / offset arithmetic.
+sub-launches of the launch planner ``_fwd_band_launches`` / ``_bwd_band_launches`` (burst_attn_interface.py) -- K/V
+blocks with carried state forward, Q-row blocks backward, views trimmed to the rows / keys each block sees.
 Here with the NATIVE kernels (tests/test_ring_gloo.py covers the same drivers with oracle ops on CPU):
 
 * public API, W=1, tiny ``BA_L2_BLOCK`` so that S ~ 1-2k already splits into many sub-launches,
