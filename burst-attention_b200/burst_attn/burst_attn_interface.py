@@ -19,6 +19,7 @@ before the round's kernel and awaited after it.
 """
 from __future__ import annotations
 
+import bisect
 import math
 import os
 from typing import List
@@ -191,10 +192,12 @@ def _merged(pieces):
     return [_sub(box, 0, qn, 0, kn)]
 
 
-def _round_pieces(layout, W, iq, jk, Sq, Sk, band, merge=True):
+def _round_pieces(layout, W, iq, jk, Sq, Sk, band, merge=True, cu=None):
     """The pieces of the round that attends the Q shard of rank ``iq`` (``Sq`` rows) to the K/V shard of rank ``jk``
     (``Sk`` keys): ``[(q0, qn, k0, kn, lo, hi)]``, rows and keys local to the shards, the band relative to the two
     views; pieces whose band misses its view are left out, and with ``merge`` exact merges are made (``_merged``).
+    ``cu``: the host list of document boundaries (``_check_cu_seqlens``), or None; each piece is then trimmed to the
+    rows and keys that share a document (``_doc_trim``), and a piece whose rows share none with its keys is left out.
     ``band`` = (left, right) counts positions in the full sequence: contiguous shards start at rank * S, zigzag shards
     are the halves rank and 2W-1-rank (one piece per pair of halves), and striped token a of rank r sits at a W + r,
     so a + ceil((iq-jk-left)/W) <= c <= a + floor((iq-jk+right)/W)."""
@@ -213,7 +216,32 @@ def _round_pieces(layout, W, iq, jk, Sq, Sk, band, merge=True):
         cand = [(qa, qn, ka, kn, None if left is None else qg - kg - left, None if right is None else qg - kg + right)
                 for qa, qn, qg in qs for ka, kn, kg in ks]
     out = [p for p in (_sub(c, 0, c[1], 0, c[3]) for c in cand) if p is not None]
+    if cu is not None:
+        pos_q, pstride = _positions(layout, W, iq, Sq)
+        pos_k, _ = _positions(layout, W, jk, Sk)
+        out = [p for p in (_doc_trim(p, cu, pos_q, pos_k, pstride) for p in out) if p is not None]
     return _merged(out) if merge else out
+
+
+def _doc_of(cu, x):
+    """The document of position x: the last d with cu[d] <= x (zero-length documents skipped), in [0, n_docs)."""
+    return bisect.bisect_right(cu, x, 0, len(cu) - 1) - 1
+
+
+def _doc_trim(piece, cu, pos_q, pos_k, pstride):
+    """A piece cut to its rows and keys in the documents both reach, or None when they share none.  Inside a piece
+    positions are affine (``pos(x0 + x) = pos(x0) + pstride x``), so the documents of its rows run from that of its first
+    row to that of its last (the same for keys), and the rows (keys) of a run of documents are one interval."""
+    qa, qn, ka, kn = piece[:4]
+    q0, k0 = pos_q(qa), pos_k(ka)
+    d0 = max(_doc_of(cu, q0), _doc_of(cu, k0))
+    d1 = min(_doc_of(cu, q0 + pstride * (qn - 1)), _doc_of(cu, k0 + pstride * (kn - 1)))
+    if d0 > d1:
+        return None
+    at = lambda p0, n, x: min(n, max(0, -((p0 - x) // pstride)))  # noqa: E731  first index at or after position x
+    r0, r1 = at(q0, qn, cu[d0]), at(q0, qn, cu[d1 + 1])
+    c0, c1 = at(k0, kn, cu[d0]), at(k0, kn, cu[d1 + 1])
+    return _sub(piece, r0, r1 - r0, c0, c1 - c0)
 
 
 def _fwd_block(piece, c0, cn):
@@ -263,6 +291,49 @@ def _bwd_band_launches(pieces):
 def _lower_kw(lo):
     """Keyword for the chunk operators: the band's lower edge (nothing without one)."""
     return {} if lo is None else {"lower": lo}
+
+
+# --------------------------------------------------------------------------- #
+# packed documents: flash-attn's cu_seqlens over positions of the full sequence
+# --------------------------------------------------------------------------- #
+def _check_cu_seqlens(cu_seqlens, S, device, name="cu_seqlens"):
+    """flash-attn's document boundaries (int32, 1-D, ``(n_docs + 1,)``, ``[0] == 0``, non-decreasing, ``[-1] == S``,
+    the length of the full sequence; repeated values are zero-length documents) -> ``(host list, device int32
+    tensor)``, or None.  The host list plans the launches and the device copy is what the kernels read; a CUDA tensor
+    costs one device-to-host copy (and synchronisation) per call, a CPU tensor one host-to-device copy."""
+    if cu_seqlens is None:
+        return None
+    if not isinstance(cu_seqlens, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor, got {type(cu_seqlens).__name__}")
+    if cu_seqlens.dtype != torch.int32:
+        raise TypeError(f"{name} must be int32, got {cu_seqlens.dtype}")
+    if cu_seqlens.dim() != 1 or cu_seqlens.numel() < 2:
+        raise ValueError(f"{name} must be 1-D with at least 2 entries (n_docs + 1), got shape {tuple(cu_seqlens.shape)}")
+    cu = cu_seqlens.tolist()
+    if cu[0] != 0 or cu[-1] != S:
+        raise ValueError(f"{name} must start at 0 and end at the sequence length {S}, got {cu[0]} .. {cu[-1]}")
+    if any(b < a for a, b in zip(cu, cu[1:])):
+        raise ValueError(f"{name} must be non-decreasing")
+    return cu, cu_seqlens.detach().to(device).contiguous()
+
+
+def _ring_doc(docs, layout, W, iq, jk, Sq, Sk):
+    """The documents of the round that attends the Q shard of rank iq to the K/V shard of rank jk: (device
+    boundaries, n_docs, pos_q, pos_k, pstride) with the position functions of ``_positions``, or None."""
+    if docs is None:
+        return None
+    pos_q, pstride = _positions(layout, W, iq, Sq)
+    pos_k, _ = _positions(layout, W, jk, Sk)
+    return docs[1], len(docs[0]) - 1, pos_q, pos_k, pstride
+
+
+def _doc_kw(doc, q0, k0):
+    """Keyword for the chunk operators: the documents of the launch whose rows start at local row q0 and keys at
+    local key k0 (nothing without documents)."""
+    if doc is None:
+        return {}
+    cu, n_docs, pos_q, pos_k, pstride = doc
+    return {"doc": (cu, n_docs, pos_q(q0), pos_k(k0), pstride)}
 
 
 # --------------------------------------------------------------------------- #
@@ -336,7 +407,7 @@ class _BandForward:
             self.o_acc.zero_()
             lse.fill_(float("-inf"))
 
-    def run(self, ops, launches, q, k, v, lse, out, scale, seq_dim, bias=None, alibi=None):
+    def run(self, ops, launches, q, k, v, lse, out, scale, seq_dim, bias=None, alibi=None, doc=None):
         for q0, qn, k0, kn, lo, hi in launches:
             first = self.first and self.done == 0
             last = self.done == self.n - 1
@@ -344,7 +415,8 @@ class _BandForward:
             ops.fwd_chunk(rows(q), k.narrow(seq_dim, k0, kn), v.narrow(seq_dim, k0, kn),
                           None if self.o_acc is None else rows(self.o_acc), lse.narrow(2, q0, qn),
                           rows(out) if last else None, scale, hi is not None, 0 if hi is None else hi, first, last,
-                          seq_dim, **_bias_kw(bias, k0, kn), **_lower_kw(lo), **_alibi_kw(alibi, q0, k0))
+                          seq_dim, **_bias_kw(bias, k0, kn), **_lower_kw(lo), **_alibi_kw(alibi, q0, k0),
+                          **_doc_kw(doc, q0, k0))
             self.done += 1
 
     def finish(self, ops, out, seq_dim):
@@ -355,13 +427,14 @@ class _BandForward:
 
 
 def _bwd_band_run(ops, launches, g, q, k, v, delta, lse, dq_part, dk_acc, dv_acc, scale, seq_dim, deterministic,
-                  bias=None, alibi=None):
+                  bias=None, alibi=None, doc=None):
     for q0, qn, k0, kn, lo, hi in launches:
         rows = lambda t: t.narrow(seq_dim, q0, qn)  # noqa: E731
         keys = lambda t: t.narrow(seq_dim, k0, kn)  # noqa: E731
         ops.bwd_chunk(rows(g), rows(q), keys(k), keys(v), delta.narrow(2, q0, qn), lse.narrow(2, q0, qn),
                       rows(dq_part), keys(dk_acc), keys(dv_acc), scale, hi is not None, 0 if hi is None else hi, seq_dim,
-                      deterministic, **_bias_kw(bias, k0, kn), **_lower_kw(lo), **_alibi_kw(alibi, q0, k0))
+                      deterministic, **_bias_kw(bias, k0, kn), **_lower_kw(lo), **_alibi_kw(alibi, q0, k0),
+                      **_doc_kw(doc, q0, k0))
 
 
 def _check_inputs(q, k, v, seq_dim):
@@ -376,7 +449,7 @@ def _check_inputs(q, k, v, seq_dim):
 # --------------------------------------------------------------------------- #
 # forward ring (reference OpBurstAttn.forward :171-253, OpBurstAttnStrip.forward :411-493)
 # --------------------------------------------------------------------------- #
-def _ring_forward(q, k, v, scale, seq_dim, layout, band, topo, alibi=None):
+def _ring_forward(q, k, v, scale, seq_dim, layout, band, topo, alibi=None, docs=None):
     """layout: the shards ("contiguous" | "zigzag" | "striped"); band: the call's (left, right) from
     ``_check_window``.  Returns (out, lse[B,H,S] fp32).  Each round runs the launches of ``_round_pieces``: the
     reference's zigzag rounds (plain causal own shard :221-224, all Q x first half of K/V :225-231, second half of Q x
@@ -391,14 +464,18 @@ def _ring_forward(q, k, v, scale, seq_dim, layout, band, topo, alibi=None):
     inter-node buffers alternate).
 
     ``alibi`` (fp32 slopes [B, H] from ``_check_alibi``) gives every launch where its rows and keys sit in the full
-    sequence; its pieces are not merged, since zigzag positions are not affine across the two halves."""
+    sequence; its pieces are not merged, since zigzag positions are not affine across the two halves.  ``docs``
+    (``_check_cu_seqlens``) does the same for packed documents, and trims every piece to its shared documents."""
     ops = get_ops()
     ring, inter, _ = topo.rings()
     L, M, W, i = topo.L, topo.M, topo.W, topo.rank
     B, S, H = q.shape[0], q.shape[seq_dim], q.shape[3 - seq_dim]
     out = torch.empty_like(q)
     lse = torch.empty((B, H, S), dtype=torch.float32, device=q.device)
-    plan = [_fwd_band_launches(_round_pieces(layout, W, i, topo.source(r), S, k.shape[seq_dim], band, alibi is None))
+    Sk = k.shape[seq_dim]
+    cu = None if docs is None else docs[0]
+    plan = [_fwd_band_launches(_round_pieces(layout, W, i, topo.source(r), S, Sk, band,
+                                             alibi is None and docs is None, cu))
             for r in range(1, W + 1)]
     state = _BandForward(plan, q, lse, S)
     if W > 1:
@@ -418,7 +495,7 @@ def _ring_forward(q, k, v, scale, seq_dim, layout, band, topo, alibi=None):
                 ring.post(cur, nxt)
             # a round whose shard lies outside every row's band launches nothing
             state.run(ops, plan[r - 1], q, cur[0], cur[1], lse, out, scale, seq_dim,
-                      alibi=_ring_alibi(alibi, layout, W, i, j, S))
+                      alibi=_ring_alibi(alibi, layout, W, i, j, S), doc=_ring_doc(docs, layout, W, i, j, S, Sk))
             if t != L - 1:
                 ring.wait()
                 cur = nxt
@@ -432,7 +509,7 @@ def _ring_forward(q, k, v, scale, seq_dim, layout, band, topo, alibi=None):
 # --------------------------------------------------------------------------- #
 # backward ring (reference OpBurstAttn.backward :256-398, OpBurstAttnStrip.backward :496-613)
 # --------------------------------------------------------------------------- #
-def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, layout, band, topo, deterministic, alibi=None):
+def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, layout, band, topo, deterministic, alibi=None, docs=None):
     """Backward of ``_ring_forward``: round r attends the Q-bundle of rank j = source(r) to the K/V at home."""
     ops = get_ops()
     W, i = topo.W, topo.rank
@@ -451,9 +528,12 @@ def _ring_backward(d_o, q, k, v, out, lse, scale, seq_dim, layout, band, topo, d
 
     def round_kernel(r, j, bundle, dq_part):
         dlt, g, qq, ls = bundle  # the bundle of rank j against the K/V at home: rows of j, keys of i
-        pieces = _round_pieces(layout, W, j, i, S, k.shape[seq_dim], band, alibi is None)
+        Sk = k.shape[seq_dim]
+        pieces = _round_pieces(layout, W, j, i, S, Sk, band, alibi is None and docs is None,
+                               None if docs is None else docs[0])
         _bwd_band_run(ops, _bwd_band_launches(pieces), g, qq, k, v, dlt, ls, dq_part, dk_acc, dv_acc, scale, seq_dim,
-                      deterministic, alibi=_ring_alibi(alibi, layout, W, j, i, S))
+                      deterministic, alibi=_ring_alibi(alibi, layout, W, j, i, S),
+                      doc=_ring_doc(docs, layout, W, j, i, S, Sk))
 
     bundle = [delta, d_o, q, lse.contiguous()]
     if W == 1:
@@ -567,10 +647,16 @@ def _bwd_rounds(ops, topo, round_kernel, bundle, q, seq_dim):
 
 # --------------------------------------------------------------------------- #
 def _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-             double_group, window_size=(-1, -1), alibi_slopes=None):
+             double_group, window_size=(-1, -1), alibi_slopes=None, cu_seqlens=None):
     assert not causal or flash == "cuda", "Causal attention only supported for Flash v2"
     ctx.band = _check_window(window_size, causal)
     ctx.alibi = _check_alibi(alibi_slopes, q, 2 if flash in ["cuda", "triton"] else 1)
+    if cu_seqlens is not None and ctx.alibi is not None:
+        raise NotImplementedError("cu_seqlens together with alibi_slopes is not supported")
+    ctx.docs = None
+    if cu_seqlens is not None:  # positions count the full sequence: W shards of the local length
+        S = q.shape[1 if flash in ["cuda", "triton"] else 2] * get_world_size(process_group)
+        ctx.docs = _check_cu_seqlens(cu_seqlens, S, q.device)
     ctx.softmax_scale = 1 / math.sqrt(q.shape[-1]) if softmax_scale is None else softmax_scale
     ctx.flash = None if flash not in ["cuda", "triton"] else flash
     ctx.seq_dim = 1 if ctx.flash else 2
@@ -612,6 +698,9 @@ def _op_forward(ctx, q, k, v, layout):
         if ctx.alibi is not None:
             raise NotImplementedError("alibi_slopes is not supported with host-resident (pinned CPU) operands; pass "
                                       "CUDA tensors")
+        if ctx.docs is not None:
+            raise NotImplementedError("cu_seqlens is not supported with host-resident (pinned CPU) operands; pass "
+                                      "CUDA tensors")
         # host-resident operands (pinned CPU tensors, one rank): copies stream under the kernels (host_stream.py)
         from . import host_stream
         if not host_stream.is_host_call(q, k, v):
@@ -624,7 +713,8 @@ def _op_forward(ctx, q, k, v, layout):
         ctx.save_for_backward(*saved)
         return o_host
     (qp, kp, vp), ctx.head_dim = _pad_head_dim(get_ops(), [q, k, v])
-    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, layout, ctx.band, ctx.topo, ctx.alibi)
+    out, lse = _ring_forward(qp, kp, vp, ctx.softmax_scale, ctx.seq_dim, layout, ctx.band, ctx.topo, ctx.alibi,
+                             ctx.docs)
     ctx.save_for_backward(qp, kp, vp, lse, out)
     return _unpad(out, ctx.head_dim)
 
@@ -634,12 +724,12 @@ def _op_backward(ctx, grad_output):
         from . import host_stream
         grads = host_stream.backward(grad_output, ctx.saved_tensors, ctx.softmax_scale, ctx.seq_dim, ctx.band,
                                      _l2_block(), ctx.deterministic)
-        return tuple(grads) + (None,) * 9
+        return tuple(grads) + (None,) * 10
     q, k, v, lse, out = ctx.saved_tensors
     (g,), _ = _pad_head_dim(get_ops(), [grad_output])
     dq, dk, dv = _ring_backward(g, q, k, v, out, lse, ctx.softmax_scale, ctx.seq_dim, ctx.layout, ctx.band, ctx.topo,
-                                ctx.deterministic, ctx.alibi)
-    return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 9
+                                ctx.deterministic, ctx.alibi, ctx.docs)
+    return tuple(_unpad(t, ctx.head_dim) for t in (dq, dk, dv)) + (None,) * 10
 
 
 class OpBurstAttn(torch.autograd.Function):
@@ -650,14 +740,17 @@ class OpBurstAttn(torch.autograd.Function):
     halves {i, 2W-1-i} when causal.  window_size: flash-attn's (left, right) sliding window over positions of
     the full sequence (-1: unlimited side; causal forces right = 0).  alibi_slopes: flash-attn's ALiBi, fp32
     (nheads,) or (batch, nheads) per query head: the bias -slope |pos_q - pos_k| over the same positions.
+    cu_seqlens: flash-attn's packed-document boundaries over the same positions (int32, ``(n_docs + 1,)``, from 0 to
+    the full sequence length, the same for every batch entry): a query sees only keys of its own document, on top of
+    causal / window_size.  Not combined with alibi_slopes (``_check_cu_seqlens`` says what it costs).
     """
 
     @staticmethod
     def forward(ctx, q, k, v, softmax_scale=None, flash="cuda", causal=False, optimize_bwd_comm=False,
                 deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1),
-                alibi_slopes=None):
+                alibi_slopes=None, cu_seqlens=None):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-                 double_group, window_size, alibi_slopes)
+                 double_group, window_size, alibi_slopes, cu_seqlens)
         return _op_forward(ctx, q, k, v, "zigzag" if causal else "contiguous")
 
     @staticmethod
@@ -672,9 +765,9 @@ class OpBurstAttnStrip(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, k, v, softmax_scale=None, flash="cuda", causal=False, optimize_bwd_comm=False,
                 deterministic=False, process_group=None, double_group=[None, None], window_size=(-1, -1),
-                alibi_slopes=None):
+                alibi_slopes=None, cu_seqlens=None):
         _prepare(ctx, q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic, process_group,
-                 double_group, window_size, alibi_slopes)
+                 double_group, window_size, alibi_slopes, cu_seqlens)
         return _op_forward(ctx, q, k, v, "striped")
 
     @staticmethod
@@ -685,14 +778,14 @@ class OpBurstAttnStrip(torch.autograd.Function):
 def burst_attn_func_striped(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: float = None,
                             flash: str = "cuda", causal: bool = False, optimize_bwd_comm: bool = False,
                             deterministic: bool = False, process_group=None, double_group=[None, None],
-                            window_size=(-1, -1), alibi_slopes=None):
+                            window_size=(-1, -1), alibi_slopes=None, cu_seqlens=None):
     return OpBurstAttnStrip.apply(q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic,
-                                  process_group, double_group, window_size, alibi_slopes)
+                                  process_group, double_group, window_size, alibi_slopes, cu_seqlens)
 
 
 def burst_attn_func(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, softmax_scale: float = None,
                     flash: str = "cuda", causal: bool = False, optimize_bwd_comm: bool = False,
                     deterministic: bool = False, process_group=None, double_group=[None, None],
-                    window_size=(-1, -1), alibi_slopes=None):
+                    window_size=(-1, -1), alibi_slopes=None, cu_seqlens=None):
     return OpBurstAttn.apply(q, k, v, softmax_scale, flash, causal, optimize_bwd_comm, deterministic,
-                             process_group, double_group, window_size, alibi_slopes)
+                             process_group, double_group, window_size, alibi_slopes, cu_seqlens)

@@ -31,6 +31,13 @@ def _alibi_args(alibi):
     return slopes.data_ptr(), slopes.stride(0), int(dist0), int(pstride)
 
 
+def _doc_args(doc):
+    """(cu_seqlens int32 device, n_docs, q_pos0, k_pos0, pstride) -> the C-ABI's arguments, in that order."""
+    cu, n_docs, q_pos0, k_pos0, pstride = doc
+    assert cu.dim() == 1 and cu.dtype == torch.int32 and cu.is_contiguous()
+    return cu.data_ptr(), int(n_docs), int(q_pos0), int(k_pos0), int(pstride)
+
+
 class NativeOps:
     name = "sm90"
     tile_head_dims = (64, 128)  # head dims the tile kernels are built for; the drivers zero-pad others up
@@ -77,12 +84,14 @@ class NativeOps:
 
     # ---- forward round: fold chunk (k, v) into (o_acc, lse); on last write o_out
     def fwd_chunk(self, q, k, v, o_acc, lse, o_out, scale, causal, causal_offset, first, last, seq_dim, bias=None,
-                  lower=None, alibi=None):
+                  lower=None, alibi=None, doc=None):
         """bias: optional fp32 [B|1, H, Sk] additive bias per key (expanded views with stride 0 over the batch are fine),
         indexed by the query head.  lower: optional lower edge of a band mask, key c visible to row a only if
         c >= a + lower (None: no lower edge).  alibi: optional ``(slopes, dist0, pstride)``, the bias
         -slopes[b, h] |pstride (a - c) + dist0| with slopes fp32 [B, H] (stride 0 over the batch is fine); not
-        combined with ``bias``."""
+        combined with ``bias``.  doc: optional ``(cu_seqlens, n_docs, q_pos0, k_pos0, pstride)``, packed documents:
+        row a (at position q_pos0 + pstride a) sees key c (at k_pos0 + pstride c) only inside one document of the
+        int32 device boundaries cu_seqlens; not combined with ``bias`` or ``alibi``."""
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         flags = (_n.BA_FWD_FIRST if first else 0) | (_n.BA_FWD_LAST if last else 0)
@@ -90,7 +99,12 @@ class NativeOps:
         args = (_n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(bias), _n.t4(o_acc, seq_dim), _n.rs(lse),
                 _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale),
                 _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
-        if alibi is not None:
+        if doc is not None:
+            assert bias is None and alibi is None, "documents are not combined with a key bias or ALiBi"
+            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
+            rc = self.lib.ba_fwd_chunk_doc(*args[:3], *args[4:-2], mask, args[-1], 0 if lower is None else int(lower),
+                                           *_doc_args(doc), flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        elif alibi is not None:
             assert bias is None, "ALiBi is not combined with a key bias"
             mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
             rc = self.lib.ba_fwd_chunk_alibi(*args[:3], *args[4:-2], mask, args[-1], 0 if lower is None else int(lower),
@@ -117,8 +131,8 @@ class NativeOps:
 
     # ---- backward round: accumulate into fp32 dq_acc / dk_acc / dv_acc
     def bwd_chunk(self, d_o, q, k, v, delta, lse, dq_acc, dk_acc, dv_acc, scale, causal, causal_offset, seq_dim,
-                  deterministic=False, bias=None, lower=None, alibi=None):
-        """lower, alibi: as in fwd_chunk."""
+                  deterministic=False, bias=None, lower=None, alibi=None, doc=None):
+        """lower, alibi, doc: as in fwd_chunk."""
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         e0 = self._t0(q.device)
@@ -126,7 +140,12 @@ class NativeOps:
                 _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv,
                 D, float(scale), _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
         tail = (1 if deterministic else 0, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
-        if alibi is not None:
+        if doc is not None:
+            assert bias is None and alibi is None, "documents are not combined with a key bias or ALiBi"
+            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
+            rc = self.lib.ba_bwd_chunk_doc(*args[:6], *args[7:-2], mask, args[-1], 0 if lower is None else int(lower),
+                                           *_doc_args(doc), *tail)
+        elif alibi is not None:
             assert bias is None, "ALiBi is not combined with a key bias"
             mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
             rc = self.lib.ba_bwd_chunk_alibi(*args[:6], *args[7:-2], mask, args[-1], 0 if lower is None else int(lower),

@@ -52,6 +52,8 @@ _EXPORTS = {
     "ba_fwd_chunk_band": (_i, [_T4, _T4, _T4, _RS, _T4, _RS, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _i, _vp]),
     "ba_fwd_chunk_alibi": (_i, [_T4, _T4, _T4, _T4, _RS, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i,
                                 _vp, _i64, _i64, _i, _i, _i, _vp]),
+    "ba_fwd_chunk_doc": (_i, [_T4, _T4, _T4, _T4, _RS, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i,
+                              _vp, _i, _i64, _i64, _i, _i, _i, _vp]),
     "ba_bwd_delta": (_i, [_T4, _T4, _RS, _i, _i, _i, _i, _i, _vp]),
     "ba_bwd_chunk": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _T4, _T4, _T4, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _vp]),
     "ba_bwd_chunk_bias": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _RS, _T4, _T4, _T4,
@@ -62,6 +64,8 @@ _EXPORTS = {
                                _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _i, _i, _vp]),
     "ba_bwd_chunk_alibi": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _T4, _T4, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i,
                                 _vp, _i64, _i64, _i, _i, _i, _vp]),
+    "ba_bwd_chunk_doc": (_i, [_T4, _T4, _T4, _T4, _RS, _RS, _T4, _T4, _T4, _i, _i, _i, _i, _i, _i, _f, _i, _i, _i,
+                              _vp, _i, _i64, _i64, _i, _i, _i, _vp]),
     "ba_cast_from_f32": (_i, [_T4, _T4, _i, _i, _i, _i, _i, _vp]),
     "ba_accumulate_f32": (_i, [_T4, _T4, _i, _i, _i, _i, _vp]),
     "ba_ring_unique_id": (_i, [_vp]),

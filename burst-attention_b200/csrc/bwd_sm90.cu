@@ -72,12 +72,14 @@ extern "C" int ba_bwd_chunk_gqa(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_t
 
 namespace ba {
 
-// ba_bwd_chunk_band and ba_bwd_chunk_alibi after their argument checks (slopes: ALiBi, else null)
+// ba_bwd_chunk_band, ba_bwd_chunk_alibi and ba_bwd_chunk_doc after their argument checks (slopes: ALiBi, else null;
+// cu: documents, else null)
 static int bwd_chunk_run(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
                          ba_rowstat key_bias, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq,
                          int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset,
                          int lower_offset, const float* slopes, int64_t slopes_stride_b, int64_t dist0, int pstride,
-                         int flags, int dtype, void* stream) {
+                         const int* cu, int n_docs, int64_t q_pos0, int64_t k_pos0, int flags, int dtype,
+                         void* stream) {
   int rc;
   BA_REQUIRE(d_o.ptr && q.ptr && k.ptr && v.ptr && delta.ptr && lse.ptr, "ba_bwd_chunk: null input");
   BA_REQUIRE(dq_acc.ptr && dk_acc.ptr && dv_acc.ptr && aligned16(dq_acc, 4) && aligned16(dk_acc, 4) &&
@@ -122,6 +124,11 @@ static int bwd_chunk_run(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 
     }
   }
   p.slopes = slopes, p.slopes_sb = slopes_stride_b, p.dist0 = dist0, p.pstride = pstride;
+  p.cu = cu, p.n_docs = n_docs, p.q_pos0 = (int)q_pos0, p.k_pos0 = (int)k_pos0;  // check_doc_args: they fit
+  if (cu) {  // the band path, with a lower edge that masks nothing when there is none (row + 1 - Sq <= 0 <= key)
+    if (!(mask_mode & BA_MASK_LOWER)) p.lo = 1 - Sq;
+    return launch_bwd_doc(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
+  }
   if (slopes) return launch_bwd_alibi(dtype, D, (mask_mode & BA_MASK_LOWER) != 0, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
   if (mask_mode & BA_MASK_LOWER) return launch_bwd_band(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
   return launch_bwd<false>(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, st);
@@ -139,7 +146,8 @@ extern "C" int ba_bwd_chunk_band(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_
                                 &lower_offset, dtype)))
     return rc;
   return ba::bwd_chunk_run(d_o, q, k, v, delta, lse, key_bias, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H_kv, D, scale,
-                           mask_mode, causal_offset, lower_offset, nullptr, 0, 0, 1, flags, dtype, stream);
+                           mask_mode, causal_offset, lower_offset, nullptr, 0, 0, 1, nullptr, 0, 0, 0, flags, dtype,
+                           stream);
 }
 
 extern "C" int ba_bwd_chunk_alibi(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
@@ -153,6 +161,21 @@ extern "C" int ba_bwd_chunk_alibi(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba
     return rc;
   ba_rowstat none = {nullptr, 0, 0};
   return ba::bwd_chunk_run(d_o, q, k, v, delta, lse, none, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H_kv, D, scale,
-                           mask_mode, causal_offset, lower_offset, slopes, slopes_stride_b, dist0, pstride, flags,
-                           dtype, stream);
+                           mask_mode, causal_offset, lower_offset, slopes, slopes_stride_b, dist0, pstride, nullptr, 0,
+                           0, 0, flags, dtype, stream);
+}
+
+extern "C" int ba_bwd_chunk_doc(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta,
+                                ba_rowstat lse, ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq,
+                                int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset,
+                                int lower_offset, const int* cu_seqlens, int n_docs, int64_t q_pos0, int64_t k_pos0,
+                                int pstride, int flags, int dtype, void* stream) {
+  int rc;
+  if ((rc = ba::check_doc_args("ba_bwd_chunk_doc", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, &causal_offset,
+                               &lower_offset, cu_seqlens, n_docs, q_pos0, k_pos0, pstride, dtype)))
+    return rc;
+  ba_rowstat none = {nullptr, 0, 0};
+  return ba::bwd_chunk_run(d_o, q, k, v, delta, lse, none, dq_acc, dk_acc, dv_acc, B, Sq, Sk, H, H_kv, D, scale,
+                           mask_mode, causal_offset, lower_offset, nullptr, 0, 0, pstride, cu_seqlens, n_docs, q_pos0,
+                           k_pos0, flags, dtype, stream);
 }

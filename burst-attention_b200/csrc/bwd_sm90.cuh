@@ -44,12 +44,18 @@
 // kBand = false is the kernel without a lower edge (bwd_sm90.cu); kBand = true lives in bwd_band_sm90.cu.
 //
 // ALiBi (kAlibi, bwd_alibi_kernel in bwd_alibi_sm90.cu): P^T gets -slope |pstride (q - c) + dist0| (see bwd_chunk_body).
+//
+// Packed documents (kDoc, bwd_doc_kernel in bwd_doc_sm90.cu; always with kBand): a key block visits only the Q blocks
+// of the documents of its first and last key, the loader stages each Q row's document keys relative to the block
+// (two int16 in [0, 128]) with the row statistics and flags a Q block whose rows do not all see the whole key block,
+// and P^T gets the per-element document mask on flagged tiles only.
 #pragma once
 #include <math.h>
 #include <stdlib.h>
 
 #include <type_traits>
 
+#include "doc_sm90.cuh"
 #include "host_common.h"
 #include "sm90_ptx.cuh"
 
@@ -85,7 +91,12 @@ struct BwdParams {
   const float* slopes;
   int64_t slopes_sb;
   int64_t dist0;
-  int pstride;
+  int pstride;  // ALiBi and kDoc: the distance in the full sequence between neighbouring rows (and keys)
+  // kDoc (appended): row a sits at position q_pos0 + pstride a, key c at k_pos0 + pstride c; both see each other only
+  // inside one document [cu[d], cu[d + 1]) of the n_docs + 1 boundaries cu (device int32; every position fits)
+  const int* cu;
+  int n_docs;
+  int q_pos0, k_pos0;
 };
 
 // ALiBi over the tile of the 64 rows from q0 and the 128 keys from k0: +1 or -1 when d has that sign (or is 0) on
@@ -132,6 +143,12 @@ struct BwdLayout {
   static constexpr int kSmemBytes = kOffBar + 64;  // no align slack: the dynamic smem base is checked to be 1 KiB aligned
   static_assert(kSmemBytes <= 232448, "backward kernel exceeds 227 KiB of shared memory");
   static_assert(kOffDQ % 1024 == 0, "SW128 dQ staging boxes need 1 KiB alignment");
+  // kDoc only, past the end of the other kernels' carve-up: per stage, each Q row's document keys relative to the
+  // key block as two int16 [lo | hi << 16], and the stage's "crosses a document edge" flag (padded to 16 bytes)
+  static constexpr int kDocStageB = kBwdM * 4 + 16;
+  static constexpr int kOffDoc = kSmemBytes;
+  static constexpr int kSmemDocBytes = kOffDoc + kBwdStages * kDocStageB;
+  static_assert(kSmemDocBytes <= 232448, "backward document kernel exceeds 227 KiB of shared memory");
 };
 
 // The kernel body; bwd_chunk_kernel (kAlibi = false) and bwd_alibi_kernel (kAlibi = true, no key bias) wrap it.
@@ -139,9 +156,10 @@ struct BwdLayout {
 // the loader folds the per-row term into the row's lse2 (it is per tile: k0 is the CTA's), and the per-key term sits
 // where the key bias goes.  On a tile that crosses d = 0, every |d| is below 192 pstride, exact in fp32, and the bias
 // is formed per element.
-template <bool kBF16, int kD, bool kBand, bool kAlibi>
+template <bool kBF16, int kD, bool kBand, bool kAlibi, bool kDoc = false>
 __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                                const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p) {
+  static_assert(!kDoc || (kBand && !kAlibi), "documents run on the band path, without ALiBi");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();  // SWIZZLE_128B atoms need a 1 KiB-aligned base
@@ -169,12 +187,22 @@ __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUt
   const int k0 = kb * kBwdN;
   const int nQ = (p.Sq + kBwdM - 1) / kBwdM;
   // first Q block that can see any key of this block: q >= k0 - off (the same for every query head of the group)
-  const int i_begin = p.causal ? max(0, k0 - p.causal_off) / kBwdM : 0;
+  int i_begin = p.causal ? max(0, k0 - p.causal_off) / kBwdM : 0;
   // band: one past the last Q block that can see any key of this block: q + lo <= min(k0 + 127, Sk - 1)
   int i_end = nQ;
   if constexpr (kBand) {
     const int q_last = min(k0 + kBwdN - 1, p.Sk - 1) - p.lo;
     i_end = q_last < 0 ? 0 : min(nQ, q_last / kBwdM + 1);
+  }
+  // documents: only the rows of the documents of the block's first and last key (documents never decrease along
+  // the keys, so these two bound the rows of every key in between)
+  if constexpr (kDoc) {
+    int r_lo, r_hi, unused;
+    doc_interval(p.k_pos0 + p.pstride * k0, p.cu, p.n_docs, p.q_pos0, p.pstride, p.Sq, &r_lo, &unused);
+    doc_interval(p.k_pos0 + p.pstride * min(k0 + kBwdN - 1, p.Sk - 1), p.cu, p.n_docs, p.q_pos0, p.pstride,
+                 p.Sq, &unused, &r_hi);
+    i_begin = max(i_begin, r_lo / kBwdM);
+    i_end = min(i_end, (r_hi + kBwdM - 1) / kBwdM);
   }
   const int n_it = max(0, i_end - i_begin);
   if (n_it == 0) return;  // nothing visible: dK/dV contributions are zero (uniform exit, no barriers yet)
@@ -235,6 +263,24 @@ __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUt
           stat[lane + 32 * j] = l * kLog2e;
         }
         stat[kBwdM + lane + 32 * j] = dl;
+      }
+      if constexpr (kDoc) {  // each row's document keys relative to k0, and whether any row misses a key of the block
+        uint32_t* dw = reinterpret_cast<uint32_t*>(smem + L::kOffDoc + st * L::kDocStageB);
+        bool cross = false;
+#pragma unroll 1
+        for (int j = 0; j < 2; ++j) {
+          const int row = q0 + lane + 32 * j;
+          int lo = 0, hi = 0;  // padding row: no key (its P is 0 anyway)
+          if (row < p.Sq) {
+            doc_interval(p.q_pos0 + p.pstride * row, p.cu, p.n_docs, p.k_pos0, p.pstride, p.Sk, &lo, &hi);
+            lo = min(max(lo - k0, 0), kBwdN);
+            hi = min(max(hi - k0, 0), kBwdN);
+            cross |= lo > 0 || hi < min(kBwdN, p.Sk - k0);
+          }
+          dw[lane + 32 * j] = (uint32_t)lo | ((uint32_t)hi << 16);
+        }
+        const unsigned any = __ballot_sync(0xffffffffu, cross);
+        if (lane == 0) dw[kBwdM] = any != 0u;
       }
       __syncwarp();
       if (lane == 0) {
@@ -314,6 +360,12 @@ __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUt
       const int q0 = (i_begin + it) * kBwdM;
       const uint32_t sQ = q_stage(st), sDO = do_stage(st);
       const float* stat = sStat + st * 2 * kBwdM;
+      [[maybe_unused]] const uint32_t* dw = nullptr;  // documents: this stage's row intervals, flag at [kBwdM]
+      [[maybe_unused]] bool need_doc = false;
+      if constexpr (kDoc) {
+        dw = reinterpret_cast<const uint32_t*>(smem + L::kOffDoc + st * L::kDocStageB);
+        need_doc = dw[kBwdM] != 0u;
+      }
       // ALiBi: the bias relative to the row term the loader folded into lse2 is ma |ka[r] + kc (q - q0)|.  One-sign
       // tile s: ma = s slope, ka = pstride (c - k0), kc = 0.  Crossing tile: ma = -slope, ka + kc (q - q0) = d, with
       // ka = pstride (q0 + 2 t - c) + dist0 (small: the 32-bit sum wraps, and its true value fits) and kc = pstride.
@@ -370,6 +422,14 @@ __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUt
             const int q = q0 + 8 * c + 2 * t;
             if (q + p.lo > keys[r]) p0 = 0.f;
             if (q + 1 + p.lo > keys[r]) p1 = 0.f;
+          }
+          if constexpr (kDoc) {
+            if (need_doc) {  // key row kr of row q is visible iff lo(q) <= kr < hi(q)
+              const uint2 iv = *reinterpret_cast<const uint2*>(dw + 8 * c + 2 * t);
+              const uint32_t kr = (uint32_t)(keys[r] - k0);
+              if (kr < (iv.x & 0xffffu) || kr >= (iv.x >> 16)) p0 = 0.f;
+              if (kr < (iv.y & 0xffffu) || kr >= (iv.y >> 16)) p1 = 0.f;
+            }
           }
           s[e] = p0, s[e + 1] = p1;
           pp[2 * c + r] = pack2<kBF16>(p0, p1);
@@ -500,10 +560,16 @@ __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUt
         if (tid == 0) {
           // deterministic mode: the fp32 adds into dq_acc[query head, q block] happen in key-block order.  Key
           // block x visits Q block i iff i_begin(x) <= i < i_end(x) (neither depends on the query head); both
-          // bounds grow with x, so the key blocks that visit Q block i are one run x_min..x_max.  Without a band's
-          // lower edge x_min = 0; with one, x visits i iff 128 x + 127 >= 64 i + lo, i.e. x_min = max(0, q0 + lo) /
-          // 128 (the last key block is cut at Sk, but if it is x_min and misses i, no key block sees i and nobody
-          // waits).  The counter starts at 0, so the turn of key block x is (x - x_min) n_red + wg: x_min's first
+          // bounds grow with x, so the key blocks that visit Q block i are one run x_min..x_max, and x_min is the
+          // least x with i_end(x) > i.  Without a band's lower edge x_min = 0; with one, i_end(x) > i iff 128 x +
+          // 127 >= 64 i + lo, i.e. x_min = max(0, q0 + lo) / 128 (the last key block is cut at Sk, but if it is x_min
+          // and misses i, no key block sees i and nobody waits).  Documents: i_end(x) is also capped by the rows of
+          // the document D of x's last key c, and that cap exceeds i iff D ends after row q0, i.e. iff D is at or
+          // after the document of row q0, i.e. iff c >= k_lo, the first key of row q0's document (doc_interval
+          // gives it, clamped to [0, Sk], from the same boundaries): the document x_min is k_lo / 128, and x_min
+          // is the larger of the two (i_end is the smaller of the two caps).  The same Sk argument holds.  Both
+          // bounds still grow with x (documents never decrease along the keys), so the run stays one run.
+          // The counter starts at 0, so the turn of key block x is (x - x_min) n_red + wg: x_min's first
           // reducer never waits, and each later one waits for x - 1, which visits i too.  Lower key blocks are
           // tickets of CTAs of the same (batch, K/V head) that started earlier (see the top of the kernel).  A CTA
           // visits its (query head, Q block) pairs once each, head-major and in increasing Q block order like every
@@ -513,6 +579,12 @@ __device__ __forceinline__ void bwd_chunk_body(const CUtensorMap& tmQ, const CUt
           int* turn = p.sem ? p.sem + ((int64_t)b * p.H + h) * nQ + (i_begin + it) : nullptr;
           int x_min = 0;
           if constexpr (kBand) x_min = max(0, q0 + p.lo) / kBwdN;
+          if constexpr (kDoc) {
+            int k_lo, unused;
+            doc_interval(p.q_pos0 + p.pstride * q0, p.cu, p.n_docs, p.k_pos0, p.pstride, p.Sk, &k_lo,
+                         &unused);
+            x_min = max(x_min, k_lo / kBwdN);
+          }
           const int my_turn = (kb - x_min) * n_red + wg;
           if (turn) {
             while (ld_acquire_gpu(turn) != my_turn) __nanosleep(64);
@@ -586,6 +658,15 @@ bwd_alibi_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   bwd_chunk_body<kBF16, kD, kBand, true>(tmQ, tmK, tmV, tmDO, tmDQ, p);
 }
 
+// document instantiations: bwd_doc_sm90.cu
+template <bool kBF16, int kD>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+bwd_doc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+               const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+               const __grid_constant__ CUtensorMap tmDQ, const BwdParams p) {
+  bwd_chunk_body<kBF16, kD, true, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, p);
+}
+
 // the kernel of one (dtype, head dim) for this TU's kBand; bwd_sm90.cu launches kBand = false,
 // bwd_band_sm90.cu (launch_bwd_band) kBand = true
 template <bool kBand>
@@ -609,5 +690,8 @@ int launch_bwd_band(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap&
 int launch_bwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
                      const CUtensorMap& tmV, const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p,
                      cudaStream_t stream);
+// bwd_doc_sm90.cu: the document kernel of (dtype, head dim)
+int launch_bwd_doc(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                   const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream);
 
 }  // namespace ba

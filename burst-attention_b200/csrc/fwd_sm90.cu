@@ -27,11 +27,13 @@ extern "C" int ba_fwd_chunk_gqa(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_row
 
 namespace ba {
 
-// ba_fwd_chunk_band and ba_fwd_chunk_alibi after their argument checks (slopes: ALiBi, else null)
+// ba_fwd_chunk_band, ba_fwd_chunk_alibi and ba_fwd_chunk_doc after their argument checks (slopes: ALiBi, else null;
+// cu: documents, else null)
 static int fwd_chunk_run(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat key_bias, ba_tensor4 o_acc,
                          ba_rowstat lse, ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
                          int mask_mode, int causal_offset, int lower_offset, const float* slopes,
-                         int64_t slopes_stride_b, int64_t dist0, int pstride, int flags, int dtype, void* stream) {
+                         int64_t slopes_stride_b, int64_t dist0, int pstride, const int* cu, int n_docs,
+                         int64_t q_pos0, int64_t k_pos0, int flags, int dtype, void* stream) {
   int rc;
   BA_REQUIRE(q.ptr && k.ptr && v.ptr && lse.ptr, "ba_fwd_chunk: null q/k/v/lse");
   const bool first = flags & BA_FWD_FIRST, last = flags & BA_FWD_LAST;
@@ -65,8 +67,13 @@ static int fwd_chunk_run(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat ke
   p.lo = lower_offset;
   p.bias = key_bias.ptr, p.bias_sb = key_bias.stride_b, p.bias_sh = key_bias.stride_h;
   p.slopes = slopes, p.slopes_sb = slopes_stride_b, p.dist0 = dist0, p.pstride = pstride;
+  p.cu = cu, p.n_docs = n_docs, p.q_pos0 = (int)q_pos0, p.k_pos0 = (int)k_pos0;  // check_doc_args: they fit
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bias = key_bias.ptr != nullptr;
+  if (cu) {  // the band path, with a lower edge that masks nothing when there is none (row + 1 - Sq <= 0 <= key)
+    if (!(mask_mode & BA_MASK_LOWER)) p.lo = 1 - Sq;
+    return launch_fwd_doc(dtype, D, tmQ, tmK, tmV, p, st);
+  }
   if (slopes) return launch_fwd_alibi(dtype, D, (mask_mode & BA_MASK_LOWER) != 0, tmQ, tmK, tmV, p, st);
   if (mask_mode & BA_MASK_LOWER) return launch_fwd_band(dtype, D, bias, tmQ, tmK, tmV, p, st);
   return launch_fwd<false>(dtype, D, bias, tmQ, tmK, tmV, p, st);
@@ -83,7 +90,7 @@ extern "C" int ba_fwd_chunk_band(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_ro
                                 &lower_offset, dtype)))
     return rc;
   return ba::fwd_chunk_run(q, k, v, key_bias, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode,
-                           causal_offset, lower_offset, nullptr, 0, 0, 1, flags, dtype, stream);
+                           causal_offset, lower_offset, nullptr, 0, 0, 1, nullptr, 0, 0, 0, flags, dtype, stream);
 }
 
 extern "C" int ba_fwd_chunk_alibi(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse,
@@ -97,5 +104,20 @@ extern "C" int ba_fwd_chunk_alibi(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_t
     return rc;
   ba_rowstat none = {nullptr, 0, 0};
   return ba::fwd_chunk_run(q, k, v, none, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset,
-                           lower_offset, slopes, slopes_stride_b, dist0, pstride, flags, dtype, stream);
+                           lower_offset, slopes, slopes_stride_b, dist0, pstride, nullptr, 0, 0, 0, flags, dtype,
+                           stream);
+}
+
+extern "C" int ba_fwd_chunk_doc(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse,
+                                ba_tensor4 o_out, int B, int Sq, int Sk, int H, int H_kv, int D, float scale,
+                                int mask_mode, int causal_offset, int lower_offset, const int* cu_seqlens, int n_docs,
+                                int64_t q_pos0, int64_t k_pos0, int pstride, int flags, int dtype, void* stream) {
+  int rc;
+  if ((rc = ba::check_doc_args("ba_fwd_chunk_doc", B, Sq, Sk, H, H_kv, D, scale, &mask_mode, &causal_offset,
+                               &lower_offset, cu_seqlens, n_docs, q_pos0, k_pos0, pstride, dtype)))
+    return rc;
+  ba_rowstat none = {nullptr, 0, 0};
+  return ba::fwd_chunk_run(q, k, v, none, o_acc, lse, o_out, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset,
+                           lower_offset, nullptr, 0, 0, pstride, cu_seqlens, n_docs, q_pos0, k_pos0, flags, dtype,
+                           stream);
 }

@@ -29,10 +29,16 @@
 // ALiBi (kAlibi, fwd_alibi_kernel in fwd_alibi_sm90.cu): the score of row a and key c gets -slope |pstride (a - c) +
 // dist0|, formed from exact integer distances relative to each row's reference (alibi_dref); tiles and masks are
 // unchanged.
+//
+// Packed documents (kDoc, fwd_doc_kernel in fwd_doc_sm90.cu; always with kBand): row a and key c see each other only
+// inside one document of cu_seqlens, on top of the band.  Within a launch positions are affine in a and c, so each
+// row's keys of its document are one interval of the view, intersected with the row's band limits; each warpgroup's
+// tile range is narrowed to the document intervals of its first and last row, and the CTA visits the hull of the two.
 #pragma once
 #include <math.h>
 #include <stdlib.h>
 
+#include "doc_sm90.cuh"
 #include "host_common.h"
 #include "sm90_ptx.cuh"
 
@@ -67,7 +73,12 @@ struct FwdParams {
   const float* slopes;
   int64_t slopes_sb;
   int64_t dist0;
-  int pstride;
+  int pstride;  // ALiBi and kDoc: the distance in the full sequence between neighbouring rows (and keys)
+  // kDoc (appended): row a sits at position q_pos0 + pstride a, key c at k_pos0 + pstride c; both see each other only
+  // inside one document [cu[d], cu[d + 1]) of the n_docs + 1 boundaries cu (device int32; every position fits)
+  const int* cu;
+  int n_docs;
+  int q_pos0, k_pos0;
 };
 
 struct __align__(8) FwdBarriers {
@@ -105,6 +116,21 @@ __device__ __forceinline__ int fwd_trip_count(int r0, const FwdParams& p) {
 // the host clamps lo to <= Sk, so r0 + lo does not overflow)
 __device__ __forceinline__ int fwd_first_tile(int r0, const FwdParams& p) { return max(0, r0 + p.lo) / kBlockN; }
 
+// kDoc: the 128-key tiles [*first, *end) the 64 Q rows starting at r0 must visit: the band's tiles narrowed to the
+// keys that share a document with the first row (from below) and the last row (from above); [0, 0) when none.
+// Documents never decrease along the rows, so these two bound the keys of every row in between.
+__device__ __forceinline__ void fwd_doc_range(int r0, const FwdParams& p, int* first, int* end) {
+  *first = *end = 0;
+  if (r0 >= p.Sq) return;
+  const int r_last = min(r0 + 63, p.Sq - 1);
+  int k_lo, k_hi, unused;
+  doc_interval(p.q_pos0 + p.pstride * r0, p.cu, p.n_docs, p.k_pos0, p.pstride, p.Sk, &k_lo, &unused);
+  doc_interval(p.q_pos0 + p.pstride * r_last, p.cu, p.n_docs, p.k_pos0, p.pstride, p.Sk, &unused, &k_hi);
+  const int f = max(fwd_first_tile(r0, p), k_lo / kBlockN);
+  const int e = min(fwd_trip_count(r0, p), (k_hi + kBlockN - 1) / kBlockN);
+  if (e > f) *first = f, *end = e;
+}
+
 // ALiBi: the smallest |d| of row a over the view's keys 0 .. Sk-1 (0 if d changes sign).  The kernel runs the row's
 // softmax relative to the bias -slope dref, so that far from d = 0 its fp32 scores stay small: a pair's score gets
 // -slope (|d| - dref), an exact integer times the slope, and only lse carries -slope dref.  A carried state lowers
@@ -126,11 +152,13 @@ __device__ __forceinline__ int64_t alibi_carried_ref(int64_t dref, float m0, flo
   return dref;
 }
 
-// The kernel body; fwd_chunk_kernel (kAlibi = false) and fwd_alibi_kernel (kAlibi = true, no key bias) wrap it.
-template <bool kBF16, int kD, bool kBias, bool kBand, bool kAlibi>
+// The kernel body; fwd_chunk_kernel (kAlibi = false), fwd_alibi_kernel (kAlibi = true, no key bias) and
+// fwd_doc_kernel (kDoc = true with kBand, no key bias) wrap it.
+template <bool kBF16, int kD, bool kBias, bool kBand, bool kAlibi, bool kDoc = false>
 __device__ __forceinline__ void fwd_chunk_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                                const FwdParams& p) {
   static_assert(!(kBias && kAlibi), "ALiBi is not combined with the key bias");
+  static_assert(!kDoc || (kBand && !kBias && !kAlibi), "documents run on the band path, without key bias or ALiBi");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();      // SWIZZLE_128B atoms need a 1 KiB-aligned base
@@ -155,6 +183,14 @@ __device__ __forceinline__ void fwd_chunk_body(const CUtensorMap& tmQ, const CUt
   if constexpr (kBand) {
     t0 = min(fwd_first_tile(row0, p), n_tiles);
     n_tiles -= t0;
+  }
+  // documents: the hull of the two warpgroups' ranges; a tile in a gap between them is skipped by both (`work`)
+  if constexpr (kDoc) {
+    int f0, e0, f1, e1;
+    fwd_doc_range(row0, p, &f0, &e0);
+    fwd_doc_range(row0 + 64, p, &f1, &e1);
+    t0 = e0 > f0 ? (e1 > f1 ? min(f0, f1) : f0) : f1;
+    n_tiles = max(0, max(e0, e1) - t0);
   }
 
   if (threadIdx.x == 0) {
@@ -224,11 +260,26 @@ __device__ __forceinline__ void fwd_chunk_body(const CUtensorMap& tmQ, const CUt
   const int w = warp & 3, g = lane >> 2, t = lane & 3;
   const int r_lo = row0 + wg * 64 + 16 * w + g;  // this thread's two rows: r_lo and r_lo + 8
   const int rows[2] = {r_lo, r_lo + 8};
-  const int n_mine = fwd_trip_count(row0 + wg * 64, p);  // this group's tiles end here (absolute tile index)
+  // documents: this group's tiles [doc_first, doc_end) (fwd_doc_range), and each row's document keys
+  [[maybe_unused]] int doc_first = 0, doc_end = 0, doc_lo[2] = {0, 0}, doc_hi[2] = {0, 0};
+  if constexpr (kDoc) {
+    fwd_doc_range(row0 + wg * 64, p, &doc_first, &doc_end);
+#pragma unroll
+    for (int r = 0; r < 2; ++r)  // a padding row (>= Sq) keeps [0, 0): its position may not fit in int32
+      if (rows[r] < p.Sq)
+        doc_interval(p.q_pos0 + p.pstride * rows[r], p.cu, p.n_docs, p.k_pos0, p.pstride, p.Sk, &doc_lo[r], &doc_hi[r]);
+  }
+  // this group's tiles end here (absolute tile index)
+  const int n_mine = kDoc ? doc_end : fwd_trip_count(row0 + wg * 64, p);
   const float scale_log2 = p.scale_log2;
   int limit[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) limit[r] = p.causal ? min(rows[r] + p.causal_off, p.Sk - 1) : p.Sk - 1;
+  // documents: each row's limits narrowed to its document's keys (a row with none keeps its carried state)
+  if constexpr (kDoc) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) limit[r] = min(limit[r], doc_hi[r] - 1);
+  }
   const int limit_min = min(limit[0], limit[1]);
   // band: this group's tiles start at my0; keys below lo_limit[r] are masked for row r
   int my0 = 0, lo_limit[2] = {0, 0};
@@ -236,6 +287,11 @@ __device__ __forceinline__ void fwd_chunk_body(const CUtensorMap& tmQ, const CUt
     my0 = fwd_first_tile(row0 + wg * 64, p);
     lo_limit[0] = rows[0] + p.lo;
     lo_limit[1] = rows[1] + p.lo;
+  }
+  if constexpr (kDoc) {
+    my0 = doc_first;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) lo_limit[r] = max(lo_limit[r], doc_lo[r]);
   }
   const int lo_limit_max = max(lo_limit[0], lo_limit[1]);
   // ALiBi: slope in log2 units, and each row's reference distance (alibi_dref)
@@ -463,6 +519,14 @@ fwd_alibi_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   fwd_chunk_body<kBF16, kD, false, kBand, true>(tmQ, tmK, tmV, p);
 }
 
+// document instantiations: fwd_doc_sm90.cu
+template <bool kBF16, int kD>
+__global__ void __launch_bounds__(kFwdThreads, 1)
+fwd_doc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+               const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
+  fwd_chunk_body<kBF16, kD, false, true, false, true>(tmQ, tmK, tmV, p);
+}
+
 // the kernel of one (dtype, head dim, bias) for this TU's kBand; fwd_sm90.cu launches kBand = false,
 // fwd_band_sm90.cu (launch_fwd_band) kBand = true
 template <bool kBand>
@@ -489,5 +553,8 @@ int launch_fwd_band(int dtype, int D, bool bias, const CUtensorMap& tmQ, const C
 // fwd_alibi_sm90.cu: the ALiBi kernel of (dtype, head dim, band)
 int launch_fwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
                      const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream);
+// fwd_doc_sm90.cu: the document kernel of (dtype, head dim)
+int launch_fwd_doc(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                   const FwdParams& p, cudaStream_t stream);
 
 }  // namespace ba

@@ -123,6 +123,24 @@ int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int
   return BA_OK;
 }
 
+int check_doc_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
+                   int* causal_offset, int* lower_offset, const int* cu_seqlens, int n_docs, int64_t q_pos0,
+                   int64_t k_pos0, int pstride, int dtype) {
+  int rc;
+  if ((rc = check_band_args(fn, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset, lower_offset, dtype)))
+    return rc;
+  BA_REQUIRE(cu_seqlens, "%s: null cu_seqlens", fn);
+  BA_REQUIRE((reinterpret_cast<uintptr_t>(cu_seqlens) & 3) == 0, "%s: cu_seqlens must be 4-byte aligned", fn);
+  BA_REQUIRE(n_docs >= 1, "%s: n_docs = %d must be >= 1", fn, n_docs);
+  BA_REQUIRE(pstride >= 1, "%s: position stride %d must be >= 1", fn, pstride);
+  BA_REQUIRE(q_pos0 >= 0 && k_pos0 >= 0, "%s: positions q_pos0 = %lld, k_pos0 = %lld must be >= 0", fn,
+             (long long)q_pos0, (long long)k_pos0);
+  // cu_seqlens is int32, so every position is; the kernels count positions in 32 bits
+  BA_REQUIRE(q_pos0 + (int64_t)pstride * (Sq - 1) <= INT32_MAX && k_pos0 + (int64_t)pstride * (Sk - 1) <= INT32_MAX,
+             "%s: the positions of the rows or keys exceed int32", fn);
+  return BA_OK;
+}
+
 }  // namespace ba
 
 #ifdef BA_SELFTEST_LIB
@@ -132,7 +150,8 @@ extern "C" const char* ba_last_error(void) { return ba::g_err; }
 // 201: grouped-query attention (ba_fwd_chunk_gqa, ba_bwd_chunk_gqa); 202: band masks (ba_fwd_chunk_band,
 // ba_bwd_chunk_band)
 // 203: ALiBi (ba_fwd_chunk_alibi, ba_bwd_chunk_alibi)
-extern "C" int ba_version(void) { return 203; }
+// 204: packed documents (ba_fwd_chunk_doc, ba_bwd_chunk_doc)
+extern "C" int ba_version(void) { return 204; }
 extern "C" int ba_device_check(void) {
   int dev = 0;
   BA_CHECK_CUDA(cudaGetDevice(&dev));

@@ -66,4 +66,10 @@ int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int
                      int* causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
                      int dtype);
 
+// The same for the document entry points: check_band_args, plus the boundaries (non-null, 4-byte aligned,
+// n_docs >= 1), pstride >= 1 and positions q_pos0, k_pos0 >= 0 whose last row and key still fit in int32.
+int check_doc_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
+                   int* causal_offset, int* lower_offset, const int* cu_seqlens, int n_docs, int64_t q_pos0,
+                   int64_t k_pos0, int pstride, int dtype);
+
 }  // namespace ba

@@ -116,6 +116,17 @@ int ba_fwd_chunk_alibi(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_ac
                        int lower_offset, const float* slopes, int64_t slopes_stride_b, int64_t dist0, int pstride,
                        int flags, int dtype, void* stream);
 
+/* Packed documents (flash-attn's cu_seqlens): ba_fwd_chunk_band without a key bias, where row i and key j also see
+ * each other only inside one document.  cu_seqlens: device int32, n_docs + 1 non-decreasing boundaries of the full
+ * sequence from cu_seqlens[0] = 0 (repeated values are zero-length documents); document d holds the positions
+ * [cu_seqlens[d], cu_seqlens[d + 1]).  Row i sits at position q_pos0 + pstride i and key j at k_pos0 + pstride j (a
+ * ring passes each launch's own; pstride is W for a striped shard, else 1).  A row with no visible key keeps its
+ * carried state (lse = -inf and O = 0 without one).  n_docs >= 1, pstride >= 1, q_pos0, k_pos0 >= 0.            */
+int ba_fwd_chunk_doc(ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_tensor4 o_acc, ba_rowstat lse, ba_tensor4 o_out,
+                     int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode, int causal_offset,
+                     int lower_offset, const int* cu_seqlens, int n_docs, int64_t q_pos0, int64_t k_pos0, int pstride,
+                     int flags, int dtype, void* stream);
+
 /* delta[b,h,s] = sum_d O[b,s,h,d] * dO[b,s,h,d]  (burst_attn_interface.py:272-278) */
 int ba_bwd_delta(ba_tensor4 o, ba_tensor4 d_o, ba_rowstat delta, int B, int S, int H, int D, int dtype,
                  void* stream);
@@ -156,6 +167,14 @@ int ba_bwd_chunk_alibi(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v,
                        ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv,
                        int D, float scale, int mask_mode, int causal_offset, int lower_offset, const float* slopes,
                        int64_t slopes_stride_b, int64_t dist0, int pstride, int flags, int dtype, void* stream);
+
+/* Packed documents: ba_bwd_chunk_band without a key bias, with the documents of ba_fwd_chunk_doc.  A key block
+ * visits only the Q blocks of its documents; keys no row shares a document with get dK = dV = 0 added.
+ * BA_BWD_DETERMINISTIC stays bitwise reproducible.                                                               */
+int ba_bwd_chunk_doc(ba_tensor4 d_o, ba_tensor4 q, ba_tensor4 k, ba_tensor4 v, ba_rowstat delta, ba_rowstat lse,
+                     ba_tensor4 dq_acc, ba_tensor4 dk_acc, ba_tensor4 dv_acc, int B, int Sq, int Sk, int H, int H_kv,
+                     int D, float scale, int mask_mode, int causal_offset, int lower_offset, const int* cu_seqlens,
+                     int n_docs, int64_t q_pos0, int64_t k_pos0, int pstride, int flags, int dtype, void* stream);
 
 /* dst[b,s,h,d] (dtype) = src[b,s,h,d] (fp32); used once per backward to hand the
  * fp32 gradient accumulators back in the input dtype.                              */
