@@ -1,14 +1,9 @@
-"""Band masks for the 16-bit model and comparator of ``tests/lowp_model.py``, and the band edge sweep.
+"""The band edge sweep of the 16-bit model and comparator of ``tests/lowp_model.py``.
 
-The band ``("band", lo, hi)`` of ``band_oracle`` (key b visible to row a iff a + lo <= b <= a + hi, None: open side)
-is what the tile kernels' band mask computes.  ``install()`` extends ``lowp_model`` in this process so that its
-masks may also be bands:
-
-* ``visible`` and ``_vis_for`` accept the band, with the model's causal mutants acting on its upper edge and the
-  faults of ``BAND_MUTANTS`` on its lower edge;
-* the fp64 chunk functions ``oracle_chain`` calls run through ``band_oracle``.
-
-Every mask lowp_model already knows keeps its own code path: the replacements hand such masks to the originals.
+The band ``("band", lo, hi)`` (key b visible to row a iff a + lo <= b <= a + hi, None: open side) is what the tile
+kernels' band mask computes; ``lowp_model`` models it, with its causal mutants acting on the band's upper edge and the
+faults of ``BAND_MUTANTS`` on its lower edge, through the kernels' index arithmetic restated there
+(``fwd_trip_count``, ``fwd_first_tile``, ``bwd_q_range``, ``host_lower``).
 
 ``BAND_SWEEP`` is the band edge sweep (tests/test_gpu_window.py runs it on the kernels, tests/test_lowp_band.py on
 the model); ``band_tile_classes`` names the edges of the kernels' tiles a case reaches, by the kernels' own index
@@ -18,8 +13,8 @@ from __future__ import annotations
 
 import torch
 
-import band_oracle as bo
 import lowp_model as lm
+from lowp_model import TILE_F, TILE_M, TILE_N, bwd_q_range, fwd_first_tile, fwd_trip_count, host_lower
 
 # One realistic fault each at the band's lower edge.  "_fwd" / "_bwd": only that kernel has the fault.
 BAND_MUTANTS = (
@@ -34,121 +29,6 @@ BAND_MUTANTS = (
     "band_drop_at_2_minus_sq",      # the host drops a lower edge of 2 - Sq, which still masks key 0 of row Sq - 1
     "band_clamp_sk_minus1",         # the host clamps lo > Sk to Sk - 1 (row 0 then sees key Sk - 1)
 )
-
-TILE_F, TILE_N, TILE_M = 128, 128, 64  # forward: 128 rows x 128 keys (two 64-row warpgroups); backward: 128 x 64
-
-_visible, _vis_for = lm.visible, lm._vis_for  # lowp_model's own
-
-
-def visible(sq, sk, mask, device=None, shift=0, strict=False, lo_shift=0):
-    """``lowp_model.visible`` extended by the band; ``lo_shift`` moves its lower edge that many keys down."""
-    if mask is None or mask[0] != "band":
-        return _visible(sq, sk, mask, device, shift=shift, strict=strict)
-    _, lo, hi = mask
-    a = torch.arange(sq, device=device).unsqueeze(1)
-    b = torch.arange(sk, device=device).unsqueeze(0)
-    m = torch.ones(sq, sk, dtype=torch.bool, device=device)
-    if lo is not None:
-        m &= b >= a + int(lo) - lo_shift
-    if hi is not None:
-        m &= (b < a + int(hi) + shift) if strict else (b <= a + int(hi) + shift)
-    return m
-
-
-# --------------------------------------------------------------------------- #
-# the kernels' index arithmetic (fwd_sm90.cuh, bwd_sm90.cuh) for one band launch
-# --------------------------------------------------------------------------- #
-def fwd_trip_count(r0, sq, sk, hi):
-    """One past the last 128-key tile the 64 rows from r0 visit (``fwd_trip_count``); hi None: not causal."""
-    if r0 >= sq:
-        return 0
-    lim = sk - 1 if hi is None else min(min(r0 + 63, sq - 1) + hi, sk - 1)
-    return 0 if lim < 0 else lim // TILE_N + 1
-
-
-def fwd_first_tile(r0, lo):
-    """The first tile the 64 rows from r0 visit (``fwd_first_tile``)."""
-    return max(0, r0 + lo) // TILE_N
-
-
-def bwd_q_range(k0, sq, sk, lo, hi):
-    """(i_begin, i_end): the 64-row Q blocks key block k0 visits (``bwd_chunk_body``)."""
-    nq = (sq + TILE_M - 1) // TILE_M
-    ib = 0 if hi is None else max(0, k0 - hi) // TILE_M
-    ql = min(k0 + TILE_N - 1, sk - 1) - lo
-    ie = 0 if ql < 0 else min(nq, ql // TILE_M + 1)
-    return ib, ie
-
-
-def host_lower(sq, sk, lo, mutant=None):
-    """The lower edge the kernels get from ``check_band_args`` (None: dropped, the kernel without one runs)."""
-    if lo is None:
-        return None
-    if lo <= (2 if mutant == "band_drop_at_2_minus_sq" else 1) - sq:
-        return None
-    if lo > sk:
-        return sk - 1 if mutant == "band_clamp_sk_minus1" else sk
-    return lo
-
-
-def vis_for(sq, sk, mask, device, mutant, side):
-    if mask is None or mask[0] != "band":
-        return _vis_for(sq, sk, mask, device, mutant, side)
-    _, lo, hi = mask
-    if mutant in ("band_drop_at_2_minus_sq", "band_clamp_sk_minus1"):
-        lo = host_lower(sq, sk, lo, mutant)
-    mask = ("band", lo, hi)
-    shift = {"causal_plus1_" + side: 1, "causal_minus1_" + side: -1}.get(mutant, 0)
-    lo_shift = {"band_lo_plus1_" + side: 1, "band_lo_minus1_" + side: -1}.get(mutant, 0)
-    vis = visible(sq, sk, mask, device, shift=shift, strict=mutant == "strict_swap", lo_shift=lo_shift)
-    if lo is None:
-        return vis
-    lo = int(lo)
-    if mutant == "band_i_end_short" and side == "bwd":
-        # per 128-key block, the last 64-row Q block it would visit contributes nothing
-        for k0 in range(0, sk, TILE_N):
-            q_last = min(k0 + TILE_N - 1, sk - 1) - lo
-            if q_last >= 0:
-                qb = min(q_last, sq - 1) // TILE_M * TILE_M
-                vis[qb:qb + TILE_M, k0:k0 + TILE_N] = False
-    if side == "fwd" and mutant in ("band_first_tile_ceil_fwd", "band_wg0_from_wg1_fwd"):
-        # the keys below the first tile a warpgroup visits are lost to its 64 rows
-        for r in range(0, sq, TILE_M):
-            if mutant == "band_first_tile_ceil_fwd":
-                t = -(-max(0, r + lo) // TILE_N)
-            else:
-                t = fwd_first_tile(r + TILE_M if r % TILE_F == 0 else r, lo)
-            vis[r:r + TILE_M, :t * TILE_N] = False
-    if mutant == "band_need_lo_first_row_bwd" and side == "bwd":
-        # on the (key block, Q block) pairs with q0 + lo <= k0 < q0 + 63 + lo the lower edge is not applied
-        free = visible(sq, sk, ("band", None, hi), device, shift=shift)
-        for k0 in range(0, sk, TILE_N):
-            ib, ie = bwd_q_range(k0, sq, sk, lo, None if hi is None else int(hi))
-            for i in range(ib, ie):
-                q0 = i * TILE_M
-                if q0 + lo <= k0 < q0 + TILE_M - 1 + lo:
-                    vis[q0:q0 + TILE_M, k0:k0 + TILE_N] = free[q0:q0 + TILE_M, k0:k0 + TILE_N]
-    return vis
-
-
-class _Oracle:
-    """``oracle.attention_oracle`` with chunk functions that also take the band."""
-
-    def __init__(self, orc):
-        self._orc = orc
-        self.chunk_forward, self.chunk_backward = bo.chunk_forward, bo.chunk_backward
-
-    def __getattr__(self, name):
-        return getattr(self._orc, name)
-
-
-def install():
-    """Extend lowp_model by the band in this process (idempotent)."""
-    if lm.visible is visible:
-        return
-    lm.visible, lm._vis_for = visible, vis_for
-    lm.orc = _Oracle(lm.orc)
-
 
 # --------------------------------------------------------------------------- #
 # the band edge sweep
@@ -349,7 +229,7 @@ def band_tile_classes(case):
             if hi is not None and lo0 == hi:
                 out.add(("host_lo", "=causal"))
         out.add(("width", "open" if hi is None or lo0 is None else hi - lo0 + 1))
-        vis = visible(sq, sk, ("band", lo0, hi))
+        vis = lm.visible(sq, sk, ("band", lo0, hi))
         sees = vis.any(1)
         lo = host_lower(sq, sk, lo0)
         carried = "carried" if c > 0 else "fresh"

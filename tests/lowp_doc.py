@@ -1,13 +1,10 @@
-"""Packed-document masks for the 16-bit model and comparator of ``tests/lowp_model.py``, and the document edge sweep.
+"""The document edge sweep of the 16-bit model and comparator of ``tests/lowp_model.py``.
 
 A document mask ``("doc", lo, hi, cu, q_pos0, k_pos0, pstride)`` is what the doc tile kernels compute for one launch:
-the band ``("band", lo, hi)`` of ``lowp_band`` (key b visible to row a iff a + lo <= b <= a + hi, None: open side), and
-row a (at position q_pos0 + pstride a) sees key b (at k_pos0 + pstride b) only inside one document ``[cu[d],
-cu[d + 1])``.  ``install()`` extends ``lowp_model`` (on top of ``lowp_band.install()``) in this process:
-
-* ``visible`` and ``_vis_for`` accept the document mask; the faults of ``DOC_MUTANTS`` act on it through the kernels'
-  own index arithmetic, restated in ``doc_index`` (a fault there is a fault of the model's visibility);
-* the fp64 chunk functions ``oracle_chain`` calls run the document mask through ``doc_oracle``.
+the band ``("band", lo, hi)`` (key b visible to row a iff a + lo <= b <= a + hi, None: open side), and row a (at
+position q_pos0 + pstride a) sees key b (at k_pos0 + pstride b) only inside one document ``[cu[d], cu[d + 1])``.
+``lowp_model`` models it; the faults of ``DOC_MUTANTS`` act there through the kernels' own index arithmetic, restated
+in ``doc_index`` (a fault there is a fault of the model's visibility).
 
 ``DOC_SWEEP`` is the document edge sweep (tests/test_gpu_varlen.py runs it on the kernels, tests/test_lowp_doc.py on
 the model); ``doc_tile_classes`` names the edges of the kernels' tiles a case reaches, by the kernels' index
@@ -18,8 +15,6 @@ from __future__ import annotations
 import torch
 
 import doc_index as di
-import doc_oracle
-import lowp_band as lb
 import lowp_model as lm
 
 # One realistic fault each.  "_fwd" / "_bwd": only that kernel has the fault.
@@ -33,115 +28,8 @@ DOC_MUTANTS = (
     "doc_search_lower_bound",       # the document search finds the first d with cu[d] >= x (both kernels)
     "doc_planner_drop_last_key",    # the planner drops a launch whose rows share a document only with its last key
 )
-# doc_index's name of each kernel fault, and the side it acts on (None: both)
-_KERNEL_FAULT = {
-    "doc_edge_plus1_fwd": ("fwd_edge_plus1", "fwd"), "doc_edge_plus1_bwd": ("bwd_edge_plus1", "bwd"),
-    "doc_edge_minus1_fwd": ("fwd_edge_minus1", "fwd"), "doc_edge_minus1_bwd": ("bwd_edge_minus1", "bwd"),
-    "doc_range_first_row_fwd": ("range_first_row_only", "fwd"), "doc_i_end_first_key_bwd": ("i_end_first_key", "bwd"),
-    "doc_search_lower_bound": ("search_lower_bound", None),
-}
 
 BF16, FP16 = torch.bfloat16, torch.float16
-
-
-def launch(sq, sk, mask):
-    """The doc_index restatement of the launch a document mask describes."""
-    _, lo, hi, cu, q_pos0, k_pos0, ps = mask
-    return di.Launch(sq, sk, hi is not None, 0 if hi is None else hi, lo, cu, q_pos0, k_pos0, ps)
-
-
-def doc_visible(sq, sk, mask, device=None, shift=0, strict=False):
-    """[sq, sk] bool: the band (with lowp_model's causal mutant hooks) and the same document."""
-    _, lo, hi, cu, q_pos0, k_pos0, ps = mask
-    band = lb.visible(sq, sk, ("band", lo, hi), device, shift=shift, strict=strict)
-    same = doc_oracle.same_doc(q_pos0 + ps * torch.arange(sq), k_pos0 + ps * torch.arange(sk), list(cu))
-    return same.to(device) & band
-
-
-def _kernel_vis(sq, sk, mask, fault, side):
-    """Visibility as the doc kernels compute it, with doc_index's ``fault``: the forward's row limits inside its
-    warpgroup's tile range, or the backward's Q-block ranges with the staged offsets and the band."""
-    L = launch(sq, sk, mask)
-    vis = torch.zeros(sq, sk, dtype=torch.bool)
-    if side == "fwd":
-        for r0 in range(0, sq, 64):
-            f, e = L.group_range(r0, fault)
-            for a in range(r0, min(r0 + 64, sq)):
-                lo, hi = L.row_limits(a, fault)
-                lo, hi = max(lo, f * di.BN), min(hi, e * di.BN - 1)
-                if lo <= hi:
-                    vis[a, lo:hi + 1] = True
-        return vis
-    c = torch.arange(sk)
-    for x in range((sk + di.BWD_N - 1) // di.BWD_N):
-        ib, ie = L.q_blocks(x, fault)
-        k0 = x * di.BWD_N
-        for a in range(ib * di.BWD_M, min(ie * di.BWD_M, sq)):
-            lo, hi = L.staged(a, x, fault)
-            blk = (c >= k0 + lo) & (c < k0 + hi) & (c >= a + L.lo)
-            if L.causal:
-                blk &= c <= a + L.off
-            vis[a] |= blk
-    return vis
-
-
-def planner_drops_last_key(sq, sk, mask):
-    """True when the planner with its last-key fault would drop this launch (``_doc_trim`` taking the keys' last
-    document from key sk - 2)."""
-    _, _, _, cu, q_pos0, k_pos0, ps = mask
-    if sk < 2:
-        return False
-    d0 = max(di.doc_of(cu, q_pos0), di.doc_of(cu, k_pos0))
-    d1 = min(di.doc_of(cu, q_pos0 + ps * (sq - 1)), di.doc_of(cu, k_pos0 + ps * (sk - 2)))
-    return d0 > d1
-
-
-def doc_vis_for(sq, sk, mask, device, mutant, side):
-    if mutant in _KERNEL_FAULT:
-        fault, only = _KERNEL_FAULT[mutant]
-        if only in (None, side):
-            return _kernel_vis(sq, sk, mask, fault, side).to(device)
-    if mutant == "doc_planner_drop_last_key" and planner_drops_last_key(sq, sk, mask):
-        return torch.zeros(sq, sk, dtype=torch.bool, device=device)
-    shift = {"causal_plus1_" + side: 1, "causal_minus1_" + side: -1}.get(mutant, 0)
-    return doc_visible(sq, sk, mask, device, shift=shift, strict=mutant == "strict_swap")
-
-
-def install():
-    """Extend lowp_model by the document mask in this process (idempotent; installs lowp_band first)."""
-    lb.install()
-    if getattr(lb._visible, "doc", False):
-        return
-    prev_visible, prev_vis_for = lb._visible, lb._vis_for
-    prev_fwd, prev_bwd = lm.orc.chunk_forward, lm.orc.chunk_backward
-
-    def visible(sq, sk, mask, device=None, shift=0, strict=False):
-        if mask is not None and mask[0] == "doc":
-            return doc_visible(sq, sk, mask, device, shift, strict)
-        return prev_visible(sq, sk, mask, device, shift=shift, strict=strict)
-
-    def vis_for(sq, sk, mask, device, mutant, side):
-        if mask is not None and mask[0] == "doc":
-            return doc_vis_for(sq, sk, mask, device, mutant, side)
-        return prev_vis_for(sq, sk, mask, device, mutant, side)
-
-    def chunk_forward(q, k, v, o_acc, lse, scale, mode, dtype=torch.float64, key_bias=None):
-        if isinstance(mode, tuple) and mode[0] == "doc":
-            assert key_bias is None
-            return doc_oracle.masked_chunk_forward(q, k, v, o_acc, lse, scale,
-                                                   doc_visible(q.shape[1], k.shape[1], mode), dtype)
-        return prev_fwd(q, k, v, o_acc, lse, scale, mode, dtype, key_bias=key_bias)
-
-    def chunk_backward(do, q, k, v, delta, lse, scale, mode, dtype=torch.float64, key_bias=None):
-        if isinstance(mode, tuple) and mode[0] == "doc":
-            assert key_bias is None
-            return doc_oracle.masked_chunk_backward(do, q, k, v, delta, lse, scale,
-                                                    doc_visible(q.shape[1], k.shape[1], mode), dtype)
-        return prev_bwd(do, q, k, v, delta, lse, scale, mode, dtype, key_bias=key_bias)
-
-    visible.doc = True
-    lb._visible, lb._vis_for = visible, vis_for
-    lm.orc.chunk_forward, lm.orc.chunk_backward = chunk_forward, chunk_backward
 
 
 # --------------------------------------------------------------------------- #
@@ -201,8 +89,8 @@ def live(case, mutant):
     """Whether the mutant changes what some chunk of the case sees, in either kernel."""
     sq = case["sq"]
     for (sk, _), m in zip(case["chunks"], case["masks"]):
-        ref = doc_visible(sq, sk, m)
-        if any(not torch.equal(doc_vis_for(sq, sk, m, None, mutant, side), ref) for side in ("fwd", "bwd")):
+        ref = lm.visible(sq, sk, m)
+        if any(not torch.equal(lm._vis_for(sq, sk, m, None, mutant, side), ref) for side in ("fwd", "bwd")):
             return True
     return False
 
@@ -232,7 +120,7 @@ def doc_tile_classes(case):
     alive0 = None
     for c, ((sk, _), m) in enumerate(zip(case["chunks"], case["masks"])):
         _, lo, hi, cu, q_pos0, k_pos0, ps = m
-        L = launch(sq, sk, m)
+        L = lm.doc_launch(sq, sk, m)
         if ps > 1:
             out.add(("pstride", ps))
         if any(a == b for a, b in zip(cu, cu[1:])):
@@ -260,7 +148,7 @@ def doc_tile_classes(case):
                 last0 = docs(cu, q_pos0 + ps * min(row0 + 63, sq - 1))
                 if docs(cu, q_pos0 + ps * (row0 + 64)) > last0:
                     out.add(("wg_split",))
-        vis = doc_visible(sq, sk, m)
+        vis = lm.visible(sq, sk, m)
         sees = vis.any(1)
         if (~sees).any():
             out.add(("dead_row",))
@@ -268,7 +156,7 @@ def doc_tile_classes(case):
             alive0 = sees
         elif (~alive0 & sees).any():
             out.add(("revived",))
-        if planner_drops_last_key(sq, sk, m) and vis.any():
+        if lm.planner_drops_last_key(sq, sk, m) and vis.any():
             out.add(("planner_last_key",))
         nQ = (sq + 63) // 64
         visits = [[] for _ in range(nQ)]

@@ -14,19 +14,27 @@
 
 The model does not reproduce the kernels' order of fp32 operations (the kernel rounds P relative to the running
 maximum of its key tile, the model relative to the final row maximum), so it is a yardstick of the same error
-magnitude, not a bitwise twin.  The truth is ``oracle/attention_oracle.py`` in fp64 on the same 16-bit inputs.
+magnitude, not a bitwise twin.  The truth is ``mask_oracle`` (``oracle/attention_oracle.py`` for the masks it states)
+in fp64 on the same 16-bit inputs.
 
-Masks follow the oracle: ``None`` or ``("causal_offset", off)`` (key b visible to row a iff ``b <= a + off``).
-Tensors are in the flash layout ``[B, S, H, D]``; K/V may have fewer heads than Q (query head h reads K/V head
-``h // G``).  Both functions run on whatever device their inputs live on.
+Masks are the kernels' (``mask_oracle.mask_of``): ``None``, ``("causal_offset", off)`` (key b visible to row a iff
+``b <= a + off``), the band ``("band", lo, hi)`` and the document mask ``("doc", lo, hi, cu, q_pos0, k_pos0, pstride)``.
+A chunk may also carry ALiBi, ``(slopes [B, H], dist0, pstride)``: ``lowp_alibi_forward`` / ``lowp_alibi_backward``
+restate the ALiBi kernels' own arithmetic, which differs from the plain kernels' (below).  Tensors are in the flash
+layout ``[B, S, H, D]``; K/V may have fewer heads than Q (query head h reads K/V head ``h // G``).  The model runs on
+whatever device its inputs live on.
 
-``mutant`` injects one realistic kernel fault into the model (``MUTANTS``); ``tests/test_lowp_model.py`` shows that
-the comparator rejects each of them.
+``mutant`` injects one realistic kernel fault into the model: ``MUTANTS`` here, ``lowp_band.BAND_MUTANTS`` at the
+band's lower edge, ``lowp_doc.DOC_MUTANTS`` in the document kernels' index arithmetic (restated in ``doc_index``) and
+``lowp_alibi.ALIBI_MUTANTS`` in the ALiBi arithmetic.  ``tests/test_lowp_{model,band,doc,alibi}.py`` show that the
+comparator rejects each of them.
 """
 from __future__ import annotations
 
 import torch
 
+import doc_index as di
+import mask_oracle as mo
 from oracle import attention_oracle as orc
 
 LOG2E = 1.4426950408889634
@@ -68,15 +76,27 @@ def _scale_log2(scale: float) -> float:
     return float(torch.tensor(scale, dtype=torch.float32) * torch.tensor(LOG2E, dtype=torch.float32))
 
 
-def visible(sq: int, sk: int, mask, device=None, shift: int = 0, strict: bool = False):
-    """[sq, sk] bool visibility of ``mask`` (None: everything visible); ``shift`` / ``strict`` are mutant hooks."""
+def visible(sq: int, sk: int, mask, device=None, shift: int = 0, strict: bool = False, lo_shift: int = 0):
+    """[sq, sk] bool visibility of ``mask`` (None: everything visible).  Mutant hooks: ``shift`` / ``strict`` act on
+    the causal offset or the band's upper edge, ``lo_shift`` moves the band's lower edge that many keys down."""
     if mask is None:
         return None
-    kind, off = mask
-    assert kind == "causal_offset", mask
     a = torch.arange(sq, device=device).unsqueeze(1)
     b = torch.arange(sk, device=device).unsqueeze(0)
-    return b < a + int(off) + shift if strict else b <= a + int(off) + shift
+    if mask[0] == "causal_offset":
+        off = int(mask[1])
+        return b < a + off + shift if strict else b <= a + off + shift
+    assert mask[0] in ("band", "doc"), mask
+    lo, hi = mask[1], mask[2]
+    m = torch.ones(sq, sk, dtype=torch.bool, device=device)
+    if lo is not None:
+        m &= b >= a + int(lo) - lo_shift
+    if hi is not None:
+        m &= (b < a + int(hi) + shift) if strict else (b <= a + int(hi) + shift)
+    if mask[0] == "doc":
+        _, _, _, cu, q_pos0, k_pos0, ps = mask
+        m &= mo.same_doc(q_pos0 + ps * torch.arange(sq), k_pos0 + ps * torch.arange(sk), list(cu)).to(device)
+    return m
 
 
 def _kv_heads(t: torch.Tensor, H: int, mutant=None) -> torch.Tensor:
@@ -110,6 +130,158 @@ def _scores_log2(q, k, scale, key_bias, mutant, side):
 
 
 def _vis_for(sq, sk, mask, device, mutant, side):
+    """``visible`` as the ``side`` ("fwd" / "bwd") kernel computes it with the fault ``mutant``."""
+    if mask is not None and mask[0] == "band":
+        return _band_vis_for(sq, sk, mask, device, mutant, side)
+    if mask is not None and mask[0] == "doc":
+        return _doc_vis_for(sq, sk, mask, device, mutant, side)
+    shift = {"causal_plus1_" + side: 1, "causal_minus1_" + side: -1}.get(mutant, 0)
+    return visible(sq, sk, mask, device, shift=shift, strict=mutant == "strict_swap")
+
+
+# --------------------------------------------------------------------------- #
+# the band kernels' index arithmetic (fwd_sm90.cuh, bwd_sm90.cuh) for one band launch, and the band's faults
+# --------------------------------------------------------------------------- #
+TILE_F, TILE_N, TILE_M = 128, 128, 64  # forward: 128 rows x 128 keys (two 64-row warpgroups); backward: 128 x 64
+
+
+def fwd_trip_count(r0, sq, sk, hi):
+    """One past the last 128-key tile the 64 rows from r0 visit (``fwd_trip_count``); hi None: not causal."""
+    if r0 >= sq:
+        return 0
+    lim = sk - 1 if hi is None else min(min(r0 + 63, sq - 1) + hi, sk - 1)
+    return 0 if lim < 0 else lim // TILE_N + 1
+
+
+def fwd_first_tile(r0, lo):
+    """The first tile the 64 rows from r0 visit (``fwd_first_tile``)."""
+    return max(0, r0 + lo) // TILE_N
+
+
+def bwd_q_range(k0, sq, sk, lo, hi):
+    """(i_begin, i_end): the 64-row Q blocks key block k0 visits (``bwd_chunk_body``)."""
+    nq = (sq + TILE_M - 1) // TILE_M
+    ib = 0 if hi is None else max(0, k0 - hi) // TILE_M
+    ql = min(k0 + TILE_N - 1, sk - 1) - lo
+    ie = 0 if ql < 0 else min(nq, ql // TILE_M + 1)
+    return ib, ie
+
+
+def host_lower(sq, sk, lo, mutant=None):
+    """The lower edge the kernels get from ``check_band_args`` (None: dropped, the kernel without one runs)."""
+    if lo is None:
+        return None
+    if lo <= (2 if mutant == "band_drop_at_2_minus_sq" else 1) - sq:
+        return None
+    if lo > sk:
+        return sk - 1 if mutant == "band_clamp_sk_minus1" else sk
+    return lo
+
+
+def _band_vis_for(sq, sk, mask, device, mutant, side):
+    """``_vis_for`` of a band: the causal mutants act on its upper edge, ``lowp_band.BAND_MUTANTS`` on its lower."""
+    _, lo, hi = mask
+    if mutant in ("band_drop_at_2_minus_sq", "band_clamp_sk_minus1"):
+        lo = host_lower(sq, sk, lo, mutant)
+    mask = ("band", lo, hi)
+    shift = {"causal_plus1_" + side: 1, "causal_minus1_" + side: -1}.get(mutant, 0)
+    lo_shift = {"band_lo_plus1_" + side: 1, "band_lo_minus1_" + side: -1}.get(mutant, 0)
+    vis = visible(sq, sk, mask, device, shift=shift, strict=mutant == "strict_swap", lo_shift=lo_shift)
+    if lo is None:
+        return vis
+    lo = int(lo)
+    if mutant == "band_i_end_short" and side == "bwd":
+        # per 128-key block, the last 64-row Q block it would visit contributes nothing
+        for k0 in range(0, sk, TILE_N):
+            q_last = min(k0 + TILE_N - 1, sk - 1) - lo
+            if q_last >= 0:
+                qb = min(q_last, sq - 1) // TILE_M * TILE_M
+                vis[qb:qb + TILE_M, k0:k0 + TILE_N] = False
+    if side == "fwd" and mutant in ("band_first_tile_ceil_fwd", "band_wg0_from_wg1_fwd"):
+        # the keys below the first tile a warpgroup visits are lost to its 64 rows
+        for r in range(0, sq, TILE_M):
+            if mutant == "band_first_tile_ceil_fwd":
+                t = -(-max(0, r + lo) // TILE_N)
+            else:
+                t = fwd_first_tile(r + TILE_M if r % TILE_F == 0 else r, lo)
+            vis[r:r + TILE_M, :t * TILE_N] = False
+    if mutant == "band_need_lo_first_row_bwd" and side == "bwd":
+        # on the (key block, Q block) pairs with q0 + lo <= k0 < q0 + 63 + lo the lower edge is not applied
+        free = visible(sq, sk, ("band", None, hi), device, shift=shift)
+        for k0 in range(0, sk, TILE_N):
+            ib, ie = bwd_q_range(k0, sq, sk, lo, None if hi is None else int(hi))
+            for i in range(ib, ie):
+                q0 = i * TILE_M
+                if q0 + lo <= k0 < q0 + TILE_M - 1 + lo:
+                    vis[q0:q0 + TILE_M, k0:k0 + TILE_N] = free[q0:q0 + TILE_M, k0:k0 + TILE_N]
+    return vis
+
+
+# --------------------------------------------------------------------------- #
+# the document kernels' faults, through their index arithmetic (doc_index)
+# --------------------------------------------------------------------------- #
+# doc_index's name of each kernel fault of lowp_doc.DOC_MUTANTS, and the side it acts on (None: both)
+_DOC_KERNEL_FAULT = {
+    "doc_edge_plus1_fwd": ("fwd_edge_plus1", "fwd"), "doc_edge_plus1_bwd": ("bwd_edge_plus1", "bwd"),
+    "doc_edge_minus1_fwd": ("fwd_edge_minus1", "fwd"), "doc_edge_minus1_bwd": ("bwd_edge_minus1", "bwd"),
+    "doc_range_first_row_fwd": ("range_first_row_only", "fwd"), "doc_i_end_first_key_bwd": ("i_end_first_key", "bwd"),
+    "doc_search_lower_bound": ("search_lower_bound", None),
+}
+
+
+def doc_launch(sq, sk, mask):
+    """The doc_index restatement of the launch a document mask describes."""
+    _, lo, hi, cu, q_pos0, k_pos0, ps = mask
+    return di.Launch(sq, sk, hi is not None, 0 if hi is None else hi, lo, cu, q_pos0, k_pos0, ps)
+
+
+def _doc_kernel_vis(sq, sk, mask, fault, side):
+    """Visibility as the doc kernels compute it, with doc_index's ``fault``: the forward's row limits inside its
+    warpgroup's tile range, or the backward's Q-block ranges with the staged offsets and the band."""
+    L = doc_launch(sq, sk, mask)
+    vis = torch.zeros(sq, sk, dtype=torch.bool)
+    if side == "fwd":
+        for r0 in range(0, sq, 64):
+            f, e = L.group_range(r0, fault)
+            for a in range(r0, min(r0 + 64, sq)):
+                lo, hi = L.row_limits(a, fault)
+                lo, hi = max(lo, f * di.BN), min(hi, e * di.BN - 1)
+                if lo <= hi:
+                    vis[a, lo:hi + 1] = True
+        return vis
+    c = torch.arange(sk)
+    for x in range((sk + di.BWD_N - 1) // di.BWD_N):
+        ib, ie = L.q_blocks(x, fault)
+        k0 = x * di.BWD_N
+        for a in range(ib * di.BWD_M, min(ie * di.BWD_M, sq)):
+            lo, hi = L.staged(a, x, fault)
+            blk = (c >= k0 + lo) & (c < k0 + hi) & (c >= a + L.lo)
+            if L.causal:
+                blk &= c <= a + L.off
+            vis[a] |= blk
+    return vis
+
+
+def planner_drops_last_key(sq, sk, mask):
+    """True when the planner with its last-key fault would drop this launch (``_doc_trim`` taking the keys' last
+    document from key sk - 2)."""
+    _, _, _, cu, q_pos0, k_pos0, ps = mask
+    if sk < 2:
+        return False
+    d0 = max(di.doc_of(cu, q_pos0), di.doc_of(cu, k_pos0))
+    d1 = min(di.doc_of(cu, q_pos0 + ps * (sq - 1)), di.doc_of(cu, k_pos0 + ps * (sk - 2)))
+    return d0 > d1
+
+
+def _doc_vis_for(sq, sk, mask, device, mutant, side):
+    """``_vis_for`` of a document mask: the causal mutants act on its band, ``lowp_doc.DOC_MUTANTS`` through the
+    kernels' (and the planner's) index arithmetic."""
+    if mutant in _DOC_KERNEL_FAULT:
+        fault, only = _DOC_KERNEL_FAULT[mutant]
+        if only in (None, side):
+            return _doc_kernel_vis(sq, sk, mask, fault, side).to(device)
+    if mutant == "doc_planner_drop_last_key" and planner_drops_last_key(sq, sk, mask):
+        return torch.zeros(sq, sk, dtype=torch.bool, device=device)
     shift = {"causal_plus1_" + side: 1, "causal_minus1_" + side: -1}.get(mutant, 0)
     return visible(sq, sk, mask, device, shift=shift, strict=mutant == "strict_swap")
 
@@ -198,43 +370,236 @@ def lowp_backward(q, k, v, do, o, lse, scale, mask=None, key_bias=None, mutant=N
 
 
 # --------------------------------------------------------------------------- #
+# ALiBi: fwd_alibi_kernel / bwd_alibi_kernel (csrc/fwd_sm90.cuh, csrc/bwd_sm90.cuh)
+# --------------------------------------------------------------------------- #
+# ``lowp_alibi_forward`` / ``lowp_alibi_backward`` restate what the ALiBi kernels compute for ``alibi = (slopes [B, H],
+# dist0, pstride)``, rounding where the kernels round (DESIGN 5.1b) and otherwise as the plain model does:
+#
+# * distances: row a and key c are ``d = pstride (a - c) + dist0`` apart, an exact int64; each row's reference ``dref``
+#   is its smallest |d| over the chunk's keys (``alibi_dref``), lowered under a live carried state of lse m0 (log2
+#   units) to the truncated fp32 ``cap = max(0, -m0) / slope2`` when that is smaller (``alibi_carried_ref``);
+# * forward: the fp32 log2 scores get ``fp32(-slope2 (|d| - dref))`` (slope2 = slope log2(e) in fp32); the carried
+#   state enters as ``m = fma(slope2, dref, m0)``; lse is ``(m + log2 l - slope2 dref) ln2``;
+# * backward, per tile of 64 rows x 128 keys from k0 (both kernels classify such tiles): on a tile where d has one
+#   sign s the loader's row statistic is ``fma(slope2, fp32(s (pstride (q - k0) + dist0)), fp32(lse log2(e)))`` and
+#   the exponent adds the per-key term ``s slope2 pstride (c - k0)``; on a tile across d = 0 it adds ``-slope2 |d|``.
+#
+# Slopes are indexed by the query head, under GQA too.  The faults of ``lowp_alibi.ALIBI_MUTANTS`` act here.
+F32 = torch.float32
+LOG2E_F = torch.tensor(LOG2E, dtype=F32)
+LN2_F = torch.tensor(LN2, dtype=F32)
+
+
+def _fma(a, b, c):
+    """fp32 fma(a, b, c) of fp32 operands: the exact product in fp64, one rounding of the sum."""
+    return (a.double() * b.double() + c.double()).to(F32)
+
+
+def slope2_of(slopes):
+    """[B, H] fp32: the slope in log2 units as the kernels load it."""
+    return slopes.to(F32) * LOG2E_F.to(slopes.device)
+
+
+def distances(sq, sk, dist0, pstride, device=None):
+    """int64 [sq, sk]: d = pstride (a - c) + dist0."""
+    a = torch.arange(sq, dtype=torch.int64, device=device).view(-1, 1)
+    c = torch.arange(sk, dtype=torch.int64, device=device).view(1, -1)
+    return pstride * (a - c) + int(dist0)
+
+
+def alibi_dref(sq, sk, dist0, pstride, device=None):
+    """int64 [sq]: each row's smallest |d| over keys 0 .. sk-1 (0 when d changes sign)."""
+    hi = pstride * torch.arange(sq, dtype=torch.int64, device=device) + int(dist0)  # d at key 0
+    lo = hi - pstride * (sk - 1)                                                    # d at key sk-1
+    return torch.maximum(lo, -hi).clamp(min=0)
+
+
+def carried_ref(dref, m0, slope2):
+    """``alibi_carried_ref``: dref [B,H,Sq] int64 lowered to trunc(max(0, -m0) / slope2) where that (fp32) is
+    smaller; m0 fp32 [B,H,Sq] (log2 units), slope2 fp32 [B,H].  Returns (dref, lowered mask)."""
+    s2 = slope2.unsqueeze(-1)
+    cap = torch.clamp(-m0, min=0.0) / torch.where(s2 > 0, s2, torch.ones_like(s2))
+    low = (s2 > 0) & (cap < dref.to(F32)) & torch.isfinite(cap)
+    return torch.where(low, cap.to(torch.int64), dref), low
+
+
+def tile_bounds(sq, sk, dist0, pstride, device=None):
+    """int64 [sq, sk]: (dmin, dmax) of the 64 x 128 tile each pair lies in, over the tile's whole geometry."""
+    R = (torch.arange(sq, dtype=torch.int64, device=device) // TILE_M * TILE_M).view(-1, 1)
+    K = (torch.arange(sk, dtype=torch.int64, device=device) // TILE_N * TILE_N).view(1, -1)
+    dmin = pstride * (R - K - (TILE_N - 1)) + int(dist0)
+    dmax = pstride * (R + TILE_M - 1 - K) + int(dist0)
+    return dmin, dmax
+
+
+def tile_sign(sq, sk, dist0, pstride, device=None, mutant=None, side="fwd"):
+    """int64 [sq, sk]: the sign the kernel gives each pair's tile, +1 / -1 (one sign, 0 counted with either) or 0
+    (across d = 0); the "sign_*" mutants misclassify the tiles one sign edge away."""
+    dmin, dmax = tile_bounds(sq, sk, dist0, pstride, device)
+    s = torch.where(dmin >= 0, 1, torch.where(dmax <= 0, -1, 0))
+    if mutant == "sign_dmin_" + side:
+        s = torch.where((dmin >= -pstride) & (dmin <= -1), 1, s)
+    if mutant == "sign_dmax_" + side:
+        s = torch.where((dmax >= 1) & (dmax <= pstride), -1, s)
+    return s
+
+
+def _alibi_of(alibi, side, mutant):
+    slopes, dist0, ps = alibi
+    return slopes, int(dist0) + (1 if mutant == "dist0_plus1_" + side else 0), int(ps)
+
+
+def lowp_alibi_forward(q, k, v, scale, mask, alibi, state=None, last=True, mutant=None, info=None):
+    """One forward chunk with carried state, rounded like ``fwd_alibi_kernel``.  Arguments and result as
+    ``lowp_model.lowp_forward``; ``alibi = (slopes fp32 [B, H], dist0, pstride)``; ``info`` (a dict), if given,
+    counts the live carried rows whose reference was lowered ("lowered") and those with dref > 0 it left alone
+    ("kept")."""
+    dtype = q.dtype
+    B, Sq, H, D = q.shape
+    Sk = k.shape[1]
+    dev = q.device
+    slopes, dist0, ps = _alibi_of(alibi, "fwd", mutant)
+    slope2 = slope2_of(slopes.to(dev))  # [B,H]
+    kk, vv = _kv_heads(k, H), _kv_heads(v, H)
+    d = distances(Sq, Sk, dist0, ps, dev)
+    sg = tile_sign(Sq, Sk, dist0, ps, dev, mutant, "fwd")
+    ad = torch.where(sg == 0, d.abs(), sg * d)  # |d| as the tile forms it
+    if mutant == "key_term_no_pstride":
+        j = torch.arange(Sk, dtype=torch.int64, device=dev).view(1, -1) % TILE_N
+        ad = torch.where(sg == 0, ad, ad + sg * (ps - 1) * j)
+    dref = alibi_dref(Sq, Sk, dist0, ps, dev).view(1, 1, Sq).expand(B, H, Sq)
+    m0 = None
+    if state is not None:
+        o0 = state[0].float().permute(0, 2, 1, 3)  # [B,H,Sq,D]
+        lse0 = state[1].float()
+        alive = lse0 != NEG_INF
+        m0 = lse0 * LOG2E_F.to(dev)
+        if mutant != "carried_not_lowered":
+            low_ref, low = carried_ref(dref, torch.where(alive, m0, torch.zeros_like(m0)), slope2)
+            dref = torch.where(alive, low_ref, dref)
+            if info is not None:
+                info["lowered"] = info.get("lowered", 0) + int((low & alive).sum())
+                info["kept"] = info.get("kept", 0) + int((~low & alive & (dref > 0)).sum())
+    dref_f = dref.to(F32)
+    x = (ad.view(1, 1, Sq, Sk) - dref.unsqueeze(-1)).to(F32)  # |d| - dref, exact integer (fp32 above 2^24)
+    bias2 = (-slope2.double().view(B, H, 1, 1) * x.double()).to(F32)
+    raw = torch.einsum("bqhd,bkhd->bhqk", q.float(), kk.float())
+    s = raw * _scale_log2(scale) + bias2
+    vis = visible(Sq, Sk, mask, dev)
+    if vis is not None:
+        s = s.masked_fill(~vis, NEG_INF)
+    m = s.amax(-1)
+    if state is not None:
+        m_c = _fma(slope2.view(B, H, 1).expand(B, H, Sq), dref_f, m0)  # m0 + slope2 dref: the row's frame
+        m = torch.where(alive, torch.maximum(m, m_c), m)
+    msafe = torch.where(m == NEG_INF, torch.zeros_like(m), m)
+    p = torch.exp2(s - msafe.unsqueeze(-1))
+    l = p.sum(-1)
+    o = torch.einsum("bhqk,bhkd->bhqd", _round(p, dtype), vv.float().permute(0, 2, 1, 3))
+    if state is not None:
+        f = torch.where(alive, torch.exp2(m_c - msafe), torch.zeros_like(m))
+        l = l + alive.float() * f
+        o = o + o0 * f.unsqueeze(-1)
+    inv = torch.where(l > 0, 1.0 / l, torch.zeros_like(l))
+    o = (o * inv.unsqueeze(-1)).permute(0, 2, 1, 3).contiguous()
+    t = m + torch.log2(torch.where(l > 0, l, torch.ones_like(l)))
+    lse = torch.where(l > 0, _fma(-slope2.view(B, H, 1).expand(B, H, Sq), dref_f, t) * LN2_F.to(dev),
+                      torch.full_like(l, NEG_INF))
+    return (o.to(dtype) if last else o), lse
+
+
+def lowp_alibi_backward(q, k, v, do, o, lse, scale, mask, alibi, mutant=None):
+    """One backward chunk, rounded like ``delta_kernel`` + ``bwd_alibi_kernel``; as ``lowp_model.lowp_backward``."""
+    dtype = q.dtype
+    B, Sq, H, D = q.shape
+    Sk, Hkv = k.shape[1], k.shape[2]
+    dev = q.device
+    slopes, dist0, ps = _alibi_of(alibi, "bwd", mutant)
+    slope2 = slope2_of(slopes.to(dev))  # [B,H]
+    slope_key = slope2
+    if mutant == "bwd_gqa_first_head":
+        G = H // Hkv
+        slope_key = slope2[:, torch.arange(H, device=dev) // G * G]
+    kk, vv = _kv_heads(k, H), _kv_heads(v, H)
+    delta = (o.float() * do.float()).sum(-1).permute(0, 2, 1)  # [B,H,Sq]
+    d = distances(Sq, Sk, dist0, ps, dev)
+    sg = tile_sign(Sq, Sk, dist0, ps, dev, mutant, "bwd")
+    a = torch.arange(Sq, dtype=torch.int64, device=dev).view(-1, 1)
+    c = torch.arange(Sk, dtype=torch.int64, device=dev).view(1, -1)
+    k0 = c // TILE_N * TILE_N
+    row_term = sg * (ps * (a - k0) + dist0)                               # 0 across d = 0
+    key_term = torch.where(sg == 0, -d.abs(), sg * ps * (c - k0))
+    lse2 = torch.where(lse == NEG_INF, torch.full_like(lse, float("inf")), lse.float()) * LOG2E_F.to(dev)
+    stat = _fma(slope2.view(B, H, 1, 1), row_term.to(F32).view(1, 1, Sq, Sk), lse2.unsqueeze(-1))
+    x0 = _fma(slope_key.view(B, H, 1, 1), key_term.to(F32).view(1, 1, Sq, Sk), -stat)
+    raw = torch.einsum("bqhd,bkhd->bhqk", q.float(), kk.float())
+    p = torch.exp2(_fma(raw, torch.tensor(_scale_log2(scale), dtype=F32), x0))
+    vis = visible(Sq, Sk, mask, dev)
+    if vis is not None:
+        p = p.masked_fill(~vis, 0.0)
+    dv = torch.einsum("bhqk,bqhd->bkhd", _round(p, dtype), do.float())
+    dp = torch.einsum("bqhd,bkhd->bhqk", do.float(), vv.float())
+    ds = _round(p * (dp - delta.unsqueeze(-1)), dtype)
+    dq = torch.einsum("bhqk,bkhd->bqhd", ds, kk.float()) * scale
+    dk = torch.einsum("bhqk,bqhd->bkhd", ds, q.float()) * scale
+    return dq, _group_sum(dk, Hkv), _group_sum(dv, Hkv)
+
+
+# --------------------------------------------------------------------------- #
 # chains of chunks: the model and the fp64 oracle side by side
 # --------------------------------------------------------------------------- #
-def lowp_chain(q, ks, vs, do, scale, masks, biases=None, mutant=None):
-    """Forward over K/V chunks ``ks[c], vs[c]`` (mask ``masks[c]``, key bias ``biases[c]``) with the fp32 state
-    carried between chunks, then the backward of every chunk against the final (O, lse).
+def lowp_chain(q, ks, vs, do, scale, masks, biases=None, mutant=None, alibis=None, lse_bwd=None, info=None):
+    """Forward over K/V chunks ``ks[c], vs[c]`` (mask ``masks[c]``, key bias ``biases[c]`` or ALiBi ``alibis[c] =
+    (slopes, dist0, pstride)``) with the fp32 state carried between chunks, then the backward of every chunk against
+    the final (O, lse).  ``info``: as in ``lowp_alibi_forward``.
+
+    ``lse_bwd``: the fp32 lse the backward reads (default: the model's own).  An ALiBi kernel test passes the kernels'
+    own: far from d = 0 the backward turns the fp32 rounding of lse itself (ulp(slope dref), DESIGN 5.1b) into an error
+    of P that the model reproduces only from the same lse; the lse is held to the oracle on its own.
     Returns dict(o, lse, states=[(o_acc, lse) after each non-last chunk], dq, dk=[per chunk], dv=[per chunk])."""
     n = len(ks)
     biases = biases or [None] * n
+    alibis = alibis or [None] * n
     state, states = None, []
     for c in range(n):
-        o, lse = lowp_forward(q, ks[c], vs[c], scale, masks[c], biases[c], state, last=c == n - 1, mutant=mutant)
+        if alibis[c] is None:
+            o, lse = lowp_forward(q, ks[c], vs[c], scale, masks[c], biases[c], state, last=c == n - 1, mutant=mutant)
+        else:
+            o, lse = lowp_alibi_forward(q, ks[c], vs[c], scale, masks[c], alibis[c], state, last=c == n - 1,
+                                        mutant=mutant, info=info)
         if c < n - 1:
             state = (o, lse)
             states.append(state)
+    lb = lse if lse_bwd is None else lse_bwd.to(q.device)
     dq = torch.zeros(q.shape, device=q.device, dtype=torch.float32)
     dks, dvs = [], []
     for c in range(n):
-        dqc, dk, dv = lowp_backward(q, ks[c], vs[c], do, o, lse, scale, masks[c], biases[c], mutant=mutant)
+        if alibis[c] is None:
+            dqc, dk, dv = lowp_backward(q, ks[c], vs[c], do, o, lb, scale, masks[c], biases[c], mutant=mutant)
+        else:
+            dqc, dk, dv = lowp_alibi_backward(q, ks[c], vs[c], do, o, lb, scale, masks[c], alibis[c], mutant=mutant)
         dq += dqc
         dks.append(dk)
         dvs.append(dv)
     return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs)
 
 
-def oracle_chain(q, ks, vs, do, scale, masks, biases=None):
-    """The same chain in fp64 with ``oracle.attention_oracle`` (on the CPU), on the same 16-bit inputs."""
+def oracle_chain(q, ks, vs, do, scale, masks, biases=None, alibis=None):
+    """The same chain in fp64 with ``mask_oracle`` (on the CPU), on the same 16-bit inputs; ALiBi enters as each
+    chunk's pair bias (``mask_oracle.chunk_bias``)."""
     n = len(ks)
-    biases = biases or [None] * n
     cpu = lambda t: None if t is None else t.detach().cpu()  # noqa: E731
     q, do = cpu(q), cpu(do)
     H, Hkv = q.shape[2], ks[0].shape[2]
     kx = [_kv_heads(cpu(k), H) for k in ks]
     vx = [_kv_heads(cpu(v), H) for v in vs]
-    modes = ["none" if m is None else m for m in masks]
+    biases = [cpu(b) for b in biases] if biases else [None] * n
+    if alibis:
+        biases = [b if a is None else mo.chunk_bias((cpu(a[0]), a[1], a[2]), q.shape[1], kx[c].shape[1])
+                  for c, (a, b) in enumerate(zip(alibis, biases))]
     o, lse, states = None, None, []
     for c in range(n):
-        o, lse = orc.chunk_forward(q, kx[c], vx[c], o, lse, scale, modes[c], key_bias=cpu(biases[c]))
+        o, lse = mo.chunk_forward(q, kx[c], vx[c], o, lse, scale, masks[c], bias=biases[c])
         if c < n - 1:
             states.append((o, lse))
     delta = orc.compute_delta(o, do)
@@ -242,12 +607,12 @@ def oracle_chain(q, ks, vs, do, scale, masks, biases=None):
     dq = torch.zeros(q.shape, dtype=torch.float64)
     dks, dvs = [], []
     for c in range(n):
-        dqc, dk, dv = orc.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, modes[c], key_bias=cpu(biases[c]))
+        dqc, dk, dv = mo.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, masks[c], bias=biases[c])
         dq += dqc
         dks.append(_group_sum(dk, Hkv))
         dvs.append(_group_sum(dv, Hkv))
     return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs,
-                **error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, [cpu(b) for b in biases], Hkv))
+                **error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, biases, Hkv))
 
 
 def error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, biases, Hkv):

@@ -8,9 +8,10 @@
   sees NaN, one that writes a source while its hop is in flight fails the snapshot check.  Several ranks can then
   share one GPU: no NCCL communicator is ever created.
 * ``run_ring_cases`` is the worker: it runs ``burst_attn_func`` / ``burst_attn_func_striped`` through autograd on
-  this rank's shard of each job, with the native kernels (or the CPU oracle, or a fault injected into either), and
-  saves O, lse, dQ, dK and dV.  ``check_ring_case`` reassembles them in the parent and compares the full sequence
-  with the fp64 oracle under the 16-bit error model of ``lowp_model``.
+  this rank's shard of each job (``ring_job``: optionally with a window, ALiBi slopes or packed documents), with the
+  native kernels (or the CPU oracle, or a fault injected into either), and saves O, lse, dQ, dK and dV.
+  ``check_ring_case`` compares the full sequence, reassembled in the parent, with the fp64 oracle under the 16-bit
+  error model of ``lowp_model``.
 """
 from __future__ import annotations
 
@@ -224,33 +225,96 @@ _LAYOUT = {"none": "contiguous", "zigzag": "zigzag", "striped": "striped"}
 
 
 def ring_job(world, mode, dtype, D, Hkv, S_local, B=2, scale="d", seq_dim=1, intra=0, dq_groups=False, l2=None,
-             det=False, fault=None):
-    """One job: ``mode`` "none" | "zigzag" | "striped" on a flat ring (``intra=0``) or a hierarchical one of nodes of
-    ``intra`` ranks, ``S_local`` rows per rank, Hq = 4 query heads, ``seq_dim`` 2 for the [B,H,S,D] layout,
-    ``l2``: BA_L2_BLOCK, ``det``: deterministic (run twice, must be bitwise equal), ``fault``: one of FAULTS."""
+             det=False, fault=None, window=None, causal=None, slopes=None, cu=None, seed=0):
+    """One job: ``mode`` "none" | "zigzag" | "striped" (the shard layout: contiguous, zigzag, striped) on a flat ring
+    (``intra=0``) or a hierarchical one of nodes of ``intra`` ranks, ``S_local`` rows per rank, Hq = 4 query heads,
+    ``seq_dim`` 2 for the [B,H,S,D] layout, ``l2``: BA_L2_BLOCK, ``det``: deterministic (run twice, must be bitwise
+    equal), ``fault``: one of FAULTS.  ``causal`` defaults to the layout's (zigzag and striped causal); striped shards
+    may also run without it.  Optional fields of the call:
+
+    * ``window``: ``window_size`` (a windowed job);
+    * ``slopes``: ALiBi slopes of shape (H,) ("h") or (B, H) ("bh"), with ``window`` (default (-1, -1));
+    * ``cu``: ``cu_seqlens`` (a document job), with ``window`` (default (-1, -1)).  Its inputs come from a generator of
+      their own seeded by ``seed``, and the library's default softmax scale, instead of ``lowp_model.make_inputs``."""
     import lowp_model as lm
+    causal = mode != "none" if causal is None else causal
+    S = S_local * world
     topo = "flat" if not intra else f"{intra}x{world // intra}" + ("dq" if dq_groups else "")
-    tag = f"ring_w{world}_{topo}_{mode}_" + ("bhsd_" if seq_dim == 2 else "") + (f"l2-{l2}_" if l2 else "") + \
-        ("det_" if det else "") + (f"{fault}_" if fault else "")
-    case = lm._case(S_local * world, [(S_local * world, None if mode == "none" else 0)], D, dtype, scale=scale, B=B,
-                    H=4, Hkv=Hkv, tag=tag)
-    return dict(id=case["id"], case=case, world=world, mode=mode, seq_dim=seq_dim, intra=intra, dq_groups=dq_groups,
-                l2=l2, det=det, fault=fault)
+    opts = ("bhsd_" if seq_dim == 2 else "") + (f"l2-{l2}_" if l2 else "") + ("det_" if det else "")
+    if (slopes is not None or cu is not None) and window is None:
+        window = (-1, -1)
+    job = dict(world=world, mode=mode, dtype=dtype, causal=causal, window=None if window is None else tuple(window),
+               slopes=slopes, cu=None if cu is None else list(cu), seed=seed, seq_dim=seq_dim, intra=intra,
+               dq_groups=dq_groups, l2=l2, det=det, fault=fault, case=None)
+    if cu is not None:
+        win = f"_win{window[0]}_{window[1]}_"
+        job["id"] = f"docring_w{world}_{topo}_{mode}{'_causal' if causal else ''}{win}{opts}n{len(cu) - 1}_s{seed}"
+        job["shape"] = (B, S, Hkv, D)
+    elif window is not None:
+        tag = f"winring_w{world}_{topo}_{mode}{'_causal' if causal else ''}_win{window[0]}_{window[1]}_{opts}"
+        job["case"] = lm._case(S, [(S, None)], D, dtype, scale=scale, B=B, H=4, Hkv=Hkv, tag=tag)
+        job["id"] = job["case"]["id"]
+        if slopes is not None:
+            job["id"] = f"alibi_{job['id']}{'bh_' if slopes == 'bh' else ''}"
+    else:
+        tag = f"ring_w{world}_{topo}_{mode}_{opts}" + (f"{fault}_" if fault else "")
+        job["case"] = lm._case(S, [(S, None if mode == "none" else 0)], D, dtype, scale=scale, B=B, H=4, Hkv=Hkv,
+                               tag=tag)
+        job["id"] = job["case"]["id"]
+    return job
+
+
+def job_inputs(job):
+    """The job's full-sequence 16-bit inputs, dict(q, ks, vs, do, scale), the same on every rank: the case's
+    (``lowp_model.make_inputs``, seeded by the case id) or a document job's own."""
+    import lowp_model as lm
+    if job["case"] is not None:
+        return lm.make_inputs(job["case"])
+    B, S, Hkv, D = job["shape"]
+    g = torch.Generator().manual_seed(job["seed"])
+    q, do = (torch.randn(B, S, 4, D, generator=g).to(job["dtype"]) for _ in range(2))
+    k, v = (torch.randn(B, S, Hkv, D, generator=g).to(job["dtype"]) for _ in range(2))
+    return dict(q=q, ks=[k], vs=[v], do=do, scale=D ** -0.5)
+
+
+def job_slopes(job):
+    """The ALiBi slopes of the call, fp32 (H,) or (B, H), or None."""
+    import mask_oracle as mo
+    if job["slopes"] is None:
+        return None
+    c = job["case"]
+    return mo.slopes_for(c["B"], c["H"], job["slopes"] == "bh", seed=1)
+
+
+def whole_mask(job):
+    """The kernels' mask of the whole sequence as one chunk (``mask_oracle.mask_of``), from the job's causal flag,
+    window and documents."""
+    if job["window"] is None:
+        return ("causal_offset", 0) if job["causal"] else None
+    left, right = job["window"]
+    lo = -left if left >= 0 else None
+    hi = 0 if job["causal"] else (right if right >= 0 else None)
+    if job["cu"] is not None:
+        return ("doc", lo, hi, tuple(job["cu"]), 0, 0, 1)
+    return None if lo is None and hi is None else ("band", lo, hi)
 
 
 def _run_job(job, rank, world, device, groups):
     """This rank's part of one job; returns (outputs in the logical [B,S,H,D] / [B,H,S] layouts, local problems)."""
-    import lowp_model as lm
     from burst_attn import burst_attn_func, burst_attn_func_striped
     from oracle import attention_oracle as orc
     mode, seq_dim, layout = job["mode"], job["seq_dim"], _LAYOUT[job["mode"]]
-    x = lm.make_inputs(job["case"])  # seeded by the case id: the same full tensors on every rank
+    x = job_inputs(job)
     lay = (lambda t: t) if seq_dim == 1 else (lambda t: t.permute(0, 2, 1, 3).contiguous())
     unlay = (lambda t: t) if seq_dim == 1 else (lambda t: t.permute(0, 2, 1, 3))
     sh = lambda t: lay(orc.shard(t, rank, world, layout)).to(device)  # noqa: E731
     q, k, v, do = sh(x["q"]), sh(x["ks"][0]), sh(x["vs"][0]), sh(x["do"])
     func = burst_attn_func_striped if mode == "striped" else burst_attn_func
     dg = groups[(job["intra"], job["dq_groups"])] if job["intra"] else [None, None]
+    scale = None if job["case"] is None else x["scale"]  # document jobs: the library's default scale
+    slopes = job_slopes(job)
+    extra = dict(window_size=job["window"] or (-1, -1), alibi_slopes=None if slopes is None else slopes.to(device),
+                 cu_seqlens=None if job["cu"] is None else torch.tensor(job["cu"], dtype=torch.int32, device=device))
     if job["l2"]:
         os.environ["BA_L2_BLOCK"] = str(job["l2"])
     else:
@@ -260,8 +324,8 @@ def _run_job(job, rank, world, device, groups):
     def call():
         qq, kk, vv = (t.clone().requires_grad_() for t in (q, k, v))
         kept = [t.detach().clone() for t in (qq, kk, vv)]
-        o = func(qq, kk, vv, x["scale"], "cuda" if seq_dim == 1 else None, mode != "none", False, job["det"], None,
-                 list(dg))
+        o = func(qq, kk, vv, scale, "cuda" if seq_dim == 1 else None, job["causal"], False, job["det"], None,
+                 list(dg), **extra)
         lse = o.grad_fn.saved_tensors[3].detach().clone()  # (q, k, v, lse, out), before grad frees them
         dq, dk, dv = torch.autograd.grad(o, (qq, kk, vv), do)
         for name, t, t0 in zip("qkv", (qq, kk, vv), kept):
@@ -350,11 +414,43 @@ def load_ring_case(job, outdir):
 def check_ring_case(job, got):
     """``got`` (``load_ring_case``) against the fp64 oracle and the 16-bit model of the whole sequence as one chunk:
     the model's error terms are sums over keys, independent of how the ring splits them, and the ring's extra
-    rounding is fp32.  Raises AssertionError."""
+    rounding is fp32.  ALiBi jobs are first held to the fp64 oracle within 2 u (O) and 4 u (the gradients), relative
+    in the Frobenius norm.  Raises AssertionError."""
+    import lowp_alibi as la
     import lowp_model as lm
-    x = lm.make_inputs(job["case"])
-    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"])
-    model = lm.lowp_chain(*args)
-    ref = lm.oracle_chain(*args)
-    absmax = lm.scores_absmax(x["q"], x["ks"], x["scale"], x["masks"])
-    lm.assert_api_within_model(job["id"], got, ref, model, job["case"]["dtype"], absmax)
+    import mask_oracle as mo
+    x = job_inputs(job)
+    masks = [whole_mask(job)]
+    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], masks)
+    dtype = job["dtype"]
+    if job["slopes"] is None:
+        model, ref = lm.lowp_chain(*args), lm.oracle_chain(*args)
+        lm.assert_api_within_model(job["id"], got, ref, model, dtype, lm.scores_absmax(x["q"], x["ks"], x["scale"],
+                                                                                      masks))
+        return
+    q, k, v, do = (t.double() for t in (x["q"], x["ks"][0], x["vs"][0], x["do"]))
+    H, Hkv = q.shape[2], k.shape[2]
+    G = H // Hkv
+    slopes = mo.as_bh(job_slopes(job), q.shape[0])
+    kx = k.repeat_interleave(G, 2)
+    o, lse, dq, dk, dv = mo.dense_attention_bwd(q, kx, v.repeat_interleave(G, 2), do, x["scale"], job["causal"],
+                                                job["window"], slopes)
+    dk, dv = (t.unflatten(2, (Hkv, G)).sum(3) for t in (dk, dv))
+    u = lm.unit_roundoff(dtype)
+    for name, ref, ku in (("o", o, 2), ("dq", dq, 4), ("dk", dk, 4), ("dv", dv, 4)):
+        e = float((got[name].double() - ref).norm() / ref.norm())
+        assert e <= ku * u, f"{job['id']} {name}: relative error {e:.3e} > {ku} u"
+    # lse: lowp_model's check, with the magnitude the fp32 score arithmetic works at (|q| |k| scale + |bias| over
+    # the keys each row sees); -inf exactly where the oracle's is
+    S = q.shape[1]
+    a = torch.einsum("bqhd,bkhd->bhqk", q.abs(), kx.abs()) * abs(x["scale"])
+    a = a - mo.bias(slopes, torch.arange(S), torch.arange(S))
+    m = mo.window_mask(S, S, job["window"], job["causal"])
+    if m is not None:
+        a = a.masked_fill(~m, 0.0)
+    lm.assert_lse(f"lse[{job['id']}]", got["lse"], lse, a.amax(-1))
+    # per (b, s, h) row against the 16-bit model of the whole sequence as one chunk: d = a - c
+    al = [(slopes.contiguous(), 0, 1)]
+    absmax = la.absmax_prefix(x["q"], x["ks"], x["scale"], masks, al)[-1]
+    lm.assert_api_within_model(job["id"], got, lm.oracle_chain(*args, alibis=al), lm.lowp_chain(*args, alibis=al),
+                               dtype, absmax)

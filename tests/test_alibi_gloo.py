@@ -1,5 +1,5 @@
 """ALiBi without a GPU: the ring drivers' per-launch distances under gloo with fp64 oracle chunk operators
-(``alibi_ops``), each run reassembled and compared with the fp64 ALiBi oracle over the full sequence; the flash_attn_*
+(``oracle_ops``), each run reassembled and compared with the fp64 ALiBi oracle over the full sequence; the flash_attn_*
 wrappers' bottom-right positions; argument checks of the public API and of the C-ABI."""
 import os
 
@@ -7,7 +7,7 @@ import pytest
 import torch
 import torch.distributed as dist
 
-import alibi_oracle as ao
+import mask_oracle as mo
 from ring_harness import double_group, spawn
 
 # window_size values: none, narrower than a shard, two-sided
@@ -34,8 +34,8 @@ def _check(rank, world, layout, window, dg=(None, None), S_local=12, Hkv=2, per_
     k, v = (torch.randn(B, S, Hkv, D, dtype=torch.float64) for _ in range(2))
     slopes = _slopes(B, H, per_batch)
     G = H // Hkv
-    o_ref, _, dq_ref, dk_ref, dv_ref = ao.dense_attention_bwd(q, k.repeat_interleave(G, 2), v.repeat_interleave(G, 2),
-                                                              do, 0.3, causal, window, ao.as_bh(slopes, B))
+    o_ref, _, dq_ref, dk_ref, dv_ref = mo.dense_attention_bwd(q, k.repeat_interleave(G, 2), v.repeat_interleave(G, 2),
+                                                              do, 0.3, causal, window, mo.as_bh(slopes, B))
     dk_ref, dv_ref = (t.unflatten(2, (Hkv, G)).sum(3) for t in (dk_ref, dv_ref))
     lay = (lambda t: t) if seq_dim == 1 else (lambda t: t.transpose(1, 2).contiguous())
     unlay = (lambda t: t) if seq_dim == 1 else (lambda t: t.transpose(1, 2))
@@ -53,8 +53,8 @@ def _check(rank, world, layout, window, dg=(None, None), S_local=12, Hkv=2, per_
 def _worker(rank, world, port, intra):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from burst_attn import chunk_ops
-    from alibi_ops import AlibiOracleOps
-    chunk_ops._set_ops_for_testing(AlibiOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         dg = double_group(rank, world, intra, False) if intra else (None, None)
         for layout in ("contiguous", "zigzag", "striped", "striped_nc"):
@@ -80,10 +80,10 @@ def test_alibi_world1_and_l2_blocks(monkeypatch, blk):
     """One rank, with and without L2 blocking (BA_L2_BLOCK = 16: sub-launches whose rows and keys start inside the
     shard, so their distance offsets shift)."""
     from burst_attn import chunk_ops
-    from alibi_ops import AlibiOracleOps
+    from oracle_ops import OracleOps
     if blk:
         monkeypatch.setenv("BA_L2_BLOCK", blk)
-    chunk_ops._set_ops_for_testing(AlibiOracleOps())
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         for layout in ("contiguous", "zigzag", "striped", "striped_nc"):
             for i, window in enumerate(WINDOWS + [(40, 3)]):
@@ -97,10 +97,10 @@ def test_flash_wrappers_alibi_cpu(monkeypatch, blk):
     """Bottom-right positions (Sq != Sk), windows, GQA and (B, H) slopes through the three wrappers."""
     from burst_attn import chunk_ops
     from burst_attn.flash_triton import flash_attn_func, flash_attn_kvpacked_func, flash_attn_qkvpacked_func
-    from alibi_ops import AlibiOracleOps
+    from oracle_ops import OracleOps
     if blk:
         monkeypatch.setenv("BA_L2_BLOCK", blk)
-    chunk_ops._set_ops_for_testing(AlibiOracleOps())
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         torch.manual_seed(9)
         tol = dict(rtol=1e-5, atol=1e-5)
@@ -114,8 +114,8 @@ def test_flash_wrappers_alibi_cpu(monkeypatch, blk):
                     o = flash_attn_func(qq, kk, vv, None, causal, 0.25, window, slopes)
                     g = torch.autograd.grad(o, (qq, kk, vv), do)
                     ke, ve = k.repeat_interleave(2, 2), v.repeat_interleave(2, 2)
-                    o_ref, _, dq, dk, dv = ao.dense_attention_bwd(q, ke, ve, do, 0.25, causal, window,
-                                                                  ao.as_bh(slopes, 2))
+                    o_ref, _, dq, dk, dv = mo.dense_attention_bwd(q, ke, ve, do, 0.25, causal, window,
+                                                                  mo.as_bh(slopes, 2))
                     torch.testing.assert_close(o.detach(), o_ref, **tol)
                     torch.testing.assert_close(g[0], dq, **tol)
                     torch.testing.assert_close(g[1], dk.unflatten(2, (2, 2)).sum(3), **tol)
@@ -125,7 +125,7 @@ def test_flash_wrappers_alibi_cpu(monkeypatch, blk):
             if sq == sk:
                 slopes = _slopes(2, 4, False)
                 o3 = flash_attn_qkvpacked_func(torch.stack([q, q, q], 2), None, True, 0.25, (9, -1), slopes)
-                ref = ao.dense_attention_bwd(q, q, q, do, 0.25, True, (9, -1), ao.as_bh(slopes, 2))[0]
+                ref = mo.dense_attention_bwd(q, q, q, do, 0.25, True, (9, -1), mo.as_bh(slopes, 2))[0]
                 torch.testing.assert_close(o3, ref, **tol)
     finally:
         chunk_ops._set_ops_for_testing(None)
@@ -135,8 +135,8 @@ def _calls_worker(rank, world, port, outdir):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from burst_attn import burst_attn_func, burst_attn_func_striped, chunk_ops
     from oracle import attention_oracle as orc
-    from alibi_ops import AlibiOracleOps
-    ops = AlibiOracleOps()
+    from oracle_ops import OracleOps
+    ops = OracleOps()
     chunk_ops._set_ops_for_testing(ops)
     try:
         torch.manual_seed(1)
@@ -162,10 +162,10 @@ def test_alibi_none_makes_todays_calls(tmp_path):
     """alibi_slopes=None records exactly the chunk calls of a call without the argument, in every layout (W = 4)."""
     spawn(_calls_worker, 4, (str(tmp_path),), timeout=300)
     for rank in range(4):
-        res = torch.load(os.path.join(tmp_path, f"calls{rank}.pt"))
+        res = torch.load(os.path.join(tmp_path, f"calls{rank}.pt"), weights_only=False)  # oracle_ops.Call records
         for name in ("contiguous", "zigzag", "striped"):
             assert res[(name, "omitted")] == res[(name, "none")], name
-            assert all(c[-1] is None for c in res[(name, "none")])
+            assert all(c.alibi is None for c in res[(name, "none")])
 
 
 @pytest.mark.parametrize("bad,exc", [(torch.tensor([0.5, 0.25], dtype=torch.float64), TypeError),
@@ -178,8 +178,8 @@ def test_alibi_none_makes_todays_calls(tmp_path):
 def test_bad_slopes_raise(bad, exc):
     from burst_attn import burst_attn_func, burst_attn_func_striped, chunk_ops
     from burst_attn.flash_triton import flash_attn_func
-    from alibi_ops import AlibiOracleOps
-    chunk_ops._set_ops_for_testing(AlibiOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         q = torch.randn(2, 8, 2, 8, dtype=torch.float64)
         for call in (lambda: burst_attn_func(q, q, q, None, "cuda", False, False, False, None, [None, None], (-1, -1),
@@ -196,8 +196,8 @@ def test_bad_slopes_raise(bad, exc):
 def test_alibi_with_key_bias_raises():
     from burst_attn import chunk_ops
     from burst_attn.flash_triton import flash_attn_func
-    from alibi_ops import AlibiOracleOps
-    chunk_ops._set_ops_for_testing(AlibiOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         q = torch.randn(1, 8, 2, 8, dtype=torch.float64)
         with pytest.raises(NotImplementedError, match="alibi_slopes"):

@@ -250,8 +250,7 @@ def test_alibi_none_is_todays_call():
 # --------------------------------------------------------------------------- #
 # chunk chains with carried state, at large positions, and faults injected into one kernel
 # --------------------------------------------------------------------------- #
-import alibi_oracle as ao  # noqa: E402
-import ring_alibi as ra  # noqa: E402
+import lowp_model as lm  # noqa: E402
 import ring_harness as rh  # noqa: E402
 
 
@@ -283,25 +282,8 @@ def _native_chain(q, ks, vs, do, scale, chunks, slopes, fwd_alibi=None, bwd_alib
 
 
 def _oracle_chain(q, ks, vs, do, scale, chunks, slopes):
-    cpu = lambda t: t.detach().cpu().double()  # noqa: E731
-    q, do = cpu(q), cpu(do)
-    H = q.shape[2]
-    G = H // ks[0].shape[2]
-    kx = [cpu(k).repeat_interleave(G, 2) for k in ks]
-    vx = [cpu(v).repeat_interleave(G, 2) for v in vs]
     masks = [("causal_offset", off) if causal else None for (causal, off), _ in chunks]
-    o = lse = None
-    for c, (_, (dist0, ps)) in enumerate(chunks):
-        o, lse = ao.chunk_forward(q, kx[c], vx[c], o, lse, scale, masks[c], (slopes.cpu(), dist0, ps))
-    delta = (o * do).sum(-1).permute(0, 2, 1)
-    lse_b = torch.where(torch.isinf(lse), torch.full_like(lse, float("inf")), lse)
-    dq, dks, dvs = torch.zeros_like(q), [], []
-    for c, (_, (dist0, ps)) in enumerate(chunks):
-        a, b, d = ao.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, masks[c], (slopes.cpu(), dist0, ps))
-        dq += a
-        dks.append(b.unflatten(2, (H // G, G)).sum(3))
-        dvs.append(d.unflatten(2, (H // G, G)).sum(3))
-    return dict(o=o, lse=lse, dq=dq, dk=dks, dv=dvs)
+    return lm.oracle_chain(q, ks, vs, do, scale, masks, alibis=[(slopes, dist0, ps) for _, (dist0, ps) in chunks])
 
 
 def _chain_errors(got, ref, dt):
@@ -397,7 +379,11 @@ def test_kernel_faults_are_rejected(chain):
 # --------------------------------------------------------------------------- #
 def _ring_jobs(world):
     S = 128 if world == 8 else 192
-    j = lambda *a, **kw: ra.alibi_job(world, *a, B=1, **kw)  # noqa: E731
+
+    def j(mode, dt, D, Hkv, S_local, window=(-1, -1), per_batch=False, **kw):
+        return rh.ring_job(world, mode, dt, D, Hkv, S_local, B=1, window=window, slopes="bh" if per_batch else "h",
+                           **kw)
+
     jobs = [j("none", BF16, 128, 2, S),
             j("zigzag", BF16, 128, 2, S, per_batch=True),
             j("striped", FP16, 64, 4, S),
@@ -422,9 +408,9 @@ RING_CASES = [j for w in RING_JOBS for j in RING_JOBS[w]]
 def runs(tmp_path_factory):
     if not torch.cuda.is_available() or torch.cuda.get_device_capability(0) != (9, 0):
         pytest.skip("needs an sm_90 GPU")
-    return ra.AlibiRuns(RING_JOBS, tmp_path_factory, timeout=900)
+    return rh.WorldRuns(RING_JOBS, "native", tmp_path_factory, timeout=900)
 
 
 @pytest.mark.parametrize("job", RING_CASES, ids=lambda j: j["id"])
 def test_ring_alibi(runs, job):
-    ra.check_alibi_case(job, rh.load_ring_case(job, runs.outdir(job["world"])))
+    rh.check_ring_case(job, rh.load_ring_case(job, runs.outdir(job["world"])))

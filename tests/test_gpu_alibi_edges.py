@@ -19,7 +19,6 @@ import torch
 pytestmark = pytest.mark.gpu
 
 import lowp_alibi as la  # noqa: E402
-import lowp_band  # noqa: E402
 import lowp_model as lm  # noqa: E402
 from burst_attn.chunk_ops import NativeOps  # noqa: E402
 
@@ -52,7 +51,7 @@ def _kw(m):
 
 
 def native_chain(x, layout, det_runs=2):
-    """The ALiBi kernels on one case: (result dict like lowp_alibi_chain's, [deterministic (dq, dks, dvs)])."""
+    """The ALiBi kernels on one case: (result dict like lowp_model.lowp_chain's, [deterministic (dq, dks, dvs)])."""
     ops = NativeOps()
     sd = 2 if layout == "normal" else 1
     q, do = _kernel_layout(x["q"], layout), _kernel_layout(x["do"], layout)
@@ -102,7 +101,7 @@ def _check_dead(x, got, ref):
     B, Sq, H = x["q"].shape[:3]
     for c, (k, m) in enumerate(zip(x["ks"], x["masks"])):
         Sk, Hkv = k.shape[1], k.shape[2]
-        vis = lowp_band.visible(Sq, Sk, m)
+        vis = lm.visible(Sq, Sk, m)
         vis = torch.ones(Sq, Sk, dtype=torch.bool) if vis is None else vis
         seen = ((~dead).unsqueeze(-1) & vis).any(2).view(B, Hkv, H // Hkv, Sk).any(2).permute(0, 2, 1)
         for name in ("dk", "dv"):
@@ -110,16 +109,16 @@ def _check_dead(x, got, ref):
 
 
 def _args(x):
-    return (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], x["alibis"])
+    return (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"])
 
 
 @pytest.mark.parametrize("case", la.ALIBI_SWEEP, ids=[c["id"] for c in la.ALIBI_SWEEP])
 def test_alibi_edges_within_model(case):
     x = la.make_alibi_inputs(case, "cuda")
     got, dets = native_chain(x, case["layout"])
-    # the model's backward reads the kernels' lse (lowp_alibi_chain); lse itself is held to the oracle below
-    model = la.lowp_alibi_chain(*_args(x), lse_bwd=got["lse"])
-    ref = la.oracle_alibi_chain(*_args(x))
+    # the model's backward reads the kernels' lse (lowp_model.lowp_chain); lse itself is held to the oracle below
+    model = lm.lowp_chain(*_args(x), alibis=x["alibis"], lse_bwd=got["lse"])
+    ref = lm.oracle_chain(*_args(x), alibis=x["alibis"])
     absmax = la.absmax_prefix(x["q"], x["ks"], x["scale"], x["masks"], x["alibis"])
     lm.assert_chain_within_model(case["id"], got, ref, model, case["dtype"], absmax)
     _check_dead(x, got, ref)
@@ -136,8 +135,8 @@ def test_alibi_edges_within_model(case):
 def test_alibi_mutant_is_rejected(mutant, case_id):
     """The comparator rejects the model with the fault, on the kernels' inputs and device."""
     x = la.make_alibi_inputs(_BY_ID[case_id], "cuda")
-    got = la.lowp_alibi_chain(*_args(x), mutant=mutant)
-    model, ref = la.lowp_alibi_chain(*_args(x)), la.oracle_alibi_chain(*_args(x))
+    got = lm.lowp_chain(*_args(x), mutant=mutant, alibis=x["alibis"])
+    model, ref = lm.lowp_chain(*_args(x), alibis=x["alibis"]), lm.oracle_chain(*_args(x), alibis=x["alibis"])
     absmax = la.absmax_prefix(x["q"], x["ks"], x["scale"], x["masks"], x["alibis"])
     worst = dict(lm.WORST)  # the rejected runs stay out of the report of the kernels' worst ratios
     try:

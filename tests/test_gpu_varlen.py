@@ -1,22 +1,18 @@
 """Packed documents (cu_seqlens) on the GPU, against the fp64 document oracle under the 16-bit error model
-(``lowp_model`` extended by ``lowp_doc``): the doc tile kernels on every case of the document edge sweep (chains of
-launches with carried state, exact zeros where nothing is attended, bitwise-reproducible deterministic mode), the
-model's document faults rejected on the same inputs, ``flash_attn_varlen_func``, and the ring at W = 2, 4 and 8 on one
-GPU (tests/ring_doc.py)."""
-import os
-
+(``lowp_model`` with the document masks of ``lowp_doc``): the doc tile kernels on every case of the document edge sweep
+(chains of launches with carried state, exact zeros where nothing is attended, bitwise-reproducible deterministic
+mode), the model's document faults rejected on the same inputs, ``flash_attn_varlen_func``, and the ring at W = 2, 4
+and 8 on one GPU (tests/ring_harness.py)."""
 import pytest
 import torch
 
 import lowp_doc
 import lowp_model as lm
-import ring_doc
 import ring_harness as rh
 
 pytestmark = pytest.mark.gpu
 
 DEV = torch.device("cuda", 0) if torch.cuda.is_available() else None
-lowp_doc.install()  # lowp_model's model, oracle chain and comparator take the document masks below
 MUTANT_CASES = lowp_doc.mutant_cases()
 
 
@@ -83,7 +79,7 @@ def _check_dead(x, got, ref):
     B, Sq, H = x["q"].shape[:3]
     for c, (k, m) in enumerate(zip(x["ks"], x["masks"])):
         Sk, Hkv = k.shape[1], k.shape[2]
-        seen = ((~dead).unsqueeze(-1) & lowp_doc.doc_visible(Sq, Sk, m)).any(2)
+        seen = ((~dead).unsqueeze(-1) & lm.visible(Sq, Sk, m)).any(2)
         seen = seen.view(B, Hkv, H // Hkv, Sk).any(2).permute(0, 2, 1)
         for name in ("dk", "dv"):
             assert (got[name][c].cpu()[~seen] == 0).all(), f"{name} of a key no row sees (chunk {c})"
@@ -153,7 +149,7 @@ def test_flash_attn_varlen_func_within_model(causal, window, monkeypatch):
     H, Hkv, D = 4, 2, 64
     q, do = (torch.randn(1, T, H, D, generator=g).to(torch.bfloat16) for _ in range(2))
     k, v = (torch.randn(1, T, Hkv, D, generator=g).to(torch.bfloat16) for _ in range(2))
-    masks = [ring_doc.whole_mask(cu, causal, window)]
+    masks = [rh.whole_mask(dict(causal=causal, window=window, cu=cu))]
     args = (q, [k], [v], do, D ** -0.5, masks)
     model, ref = lm.lowp_chain(*args), lm.oracle_chain(*args)
     absmax = lm.scores_absmax(q, [k], D ** -0.5, masks)
@@ -175,39 +171,32 @@ def _jobs():
     for world in (2, 4, 8):
         S_local = 256
         S = S_local * world
+
+        def j(mode, cu, D=128, **kw):
+            return rh.ring_job(world, mode, torch.bfloat16, D, 2, S_local, cu=cu, **kw)
+
         cus = [[0, S], [0, 300, 301, 301, S - 129, S], list(range(0, S, 200)) + [S],
                [0, 127, 128, 129, 255, 256, 257, 511, 512, S]]
         for mode in ("none", "zigzag", "striped"):
             for n, cu in enumerate(cus):
-                jobs.setdefault(world, []).append(ring_doc.doc_job(world, mode, cu, seed=n, D=128 if n % 2 else 64))
-            jobs[world].append(ring_doc.doc_job(world, mode, cus[1], window=(150, -1), seed=9,
-                                                seq_dim=2 if mode == "none" else 1))
-        jobs[world].append(ring_doc.doc_job(world, "striped", cus[2], causal=False, seed=7))
-        jobs[world].append(ring_doc.doc_job(world, "zigzag", cus[3], det=True, seed=8))
+                jobs.setdefault(world, []).append(j(mode, cu, seed=n, D=128 if n % 2 else 64))
+            jobs[world].append(j(mode, cus[1], window=(150, -1), seed=9, seq_dim=2 if mode == "none" else 1))
+        jobs[world].append(j("striped", cus[2], causal=False, seed=7))
+        jobs[world].append(j("zigzag", cus[3], det=True, seed=8))
         if world >= 4:
             for mode in ("none", "zigzag", "striped"):
-                jobs[world].append(ring_doc.doc_job(world, mode, cus[1], intra=2, seed=10))
+                jobs[world].append(j(mode, cus[1], intra=2, seed=10))
     return jobs
 
 
 JOBS = _jobs()
-_RUNS = {}
 
 
-def _outdir(world, tmp_path_factory):
-    if world not in _RUNS:
-        out = str(tmp_path_factory.mktemp(f"docring_w{world}"))
-        try:
-            rh.spawn(ring_doc.run_doc_cases, world, (JOBS[world], out), timeout=900)
-            _RUNS[world] = (out, None)
-        except BaseException as e:  # noqa: BLE001
-            _RUNS[world] = (None, e)
-    out, err = _RUNS[world]
-    if err is not None:
-        raise RuntimeError(f"the W={world} ranks failed: {err}")
-    return out
+@pytest.fixture(scope="module")
+def runs(tmp_path_factory):
+    return rh.WorldRuns(JOBS, "native", tmp_path_factory, timeout=900)
 
 
 @pytest.mark.parametrize("job", [j for w in sorted(JOBS) for j in JOBS[w]], ids=lambda j: j["id"])
-def test_doc_ring_on_one_device(job, tmp_path_factory):
-    ring_doc.load_and_check(job, _outdir(job["world"], tmp_path_factory))
+def test_doc_ring_on_one_device(job, runs):
+    rh.check_ring_case(job, rh.load_ring_case(job, runs.outdir(job["world"])))

@@ -14,23 +14,21 @@
 * Causal offsets at the ends of the C-ABI's int range give what the nearest in-range offsets (Sk, -Sq) give.
 * ``flash_attn_func`` / ``_kvpacked_func`` / ``_qkvpacked_func`` with ``window_size``, causal and not, Sq != Sk, with
   BA_L2_BLOCK = 256 so that rows whose first visible key block is not block 0 start their state in later launches.
-* The ring at W = 2, 4 and 8 on one device (``ring_band`` over ``ring_harness``), flat and hierarchical, in all three shard layouts.
+* The ring at W = 2, 4 and 8 on one device (``ring_harness``), flat and hierarchical, in all three shard layouts.
 """
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
 
-import band_oracle as bo  # noqa: E402
 import lowp_band  # noqa: E402
 import lowp_model as lm  # noqa: E402
-import ring_band as rb  # noqa: E402
+import mask_oracle as mo  # noqa: E402
 import ring_harness as rh  # noqa: E402
 from burst_attn.flash_triton import flash_attn_func, flash_attn_kvpacked_func, flash_attn_qkvpacked_func  # noqa: E402
 from burst_attn.chunk_ops import NativeOps  # noqa: E402
 
 BF16, FP16 = torch.bfloat16, torch.float16
-lowp_band.install()  # lowp_model's model, oracle chain and comparator take the band masks below
 _BY_ID = {c["id"]: c for c in lowp_band.BAND_SWEEP}
 
 
@@ -111,7 +109,7 @@ def _check_dead(x, got, ref):
     B, Sq, H = x["q"].shape[:3]
     for c, (k, m) in enumerate(zip(x["ks"], x["masks"])):
         Sk, Hkv = k.shape[1], k.shape[2]
-        seen = (~dead).unsqueeze(-1) & lowp_band.visible(Sq, Sk, m)
+        seen = (~dead).unsqueeze(-1) & lm.visible(Sq, Sk, m)
         if x["biases"][c] is not None:
             seen = seen & ~torch.isinf(x["biases"][c].cpu()).unsqueeze(2)
         seen = seen.any(2).view(B, Hkv, H // Hkv, Sk).any(2).permute(0, 2, 1)
@@ -242,7 +240,7 @@ def test_flash_wrappers_window(monkeypatch, fn, causal, window, sq, sk, l2):
     lm.assert_api_within_model(case["id"], dict(o=o, dq=dq, dk=dk, dv=dv), lm.oracle_chain(*args),
                                lm.lowp_chain(*args), BF16)
     # cross-check the band against flash-attn's window convention in the dense oracle
-    o_ref, _ = bo.dense_attention(q.cpu(), k.cpu(), v.cpu(), x["scale"], causal, window)
+    o_ref, _ = mo.dense_attention(q.cpu(), k.cpu(), v.cpu(), x["scale"], causal, window)
     torch.testing.assert_close(o.float().cpu(), o_ref.float(), rtol=2e-2, atol=2e-2)
 
 
@@ -251,7 +249,10 @@ def test_flash_wrappers_window(monkeypatch, fn, causal, window, sq, sk, l2):
 # --------------------------------------------------------------------------- #
 def _ring_jobs(world):
     S = 128 if world == 8 else 192
-    j = lambda *a, **kw: rb.window_job(world, *a, B=1, **kw)  # noqa: E731
+
+    def j(mode, dt, D, Hkv, S_local, window, **kw):
+        return rh.ring_job(world, mode, dt, D, Hkv, S_local, B=1, window=window, **kw)
+
     jobs = [j("none", BF16, 128, 2, S, (S // 2, S // 2)),               # spans neighbouring shards only
             j("zigzag", BF16, 128, 2, S, (S + 40, -1)),                 # spans several halves
             j("striped", FP16, 64, 4, S, (37, -1)),
@@ -273,12 +274,12 @@ RING_CASES = [j for w in RING_JOBS for j in RING_JOBS[w]]
 def runs(tmp_path_factory):
     if not torch.cuda.is_available() or torch.cuda.get_device_capability(0) != (9, 0):
         pytest.skip("needs an sm_90 GPU")
-    return rb.WindowRuns(RING_JOBS, tmp_path_factory, timeout=900)
+    return rh.WorldRuns(RING_JOBS, "native", tmp_path_factory, timeout=900)
 
 
 @pytest.mark.parametrize("job", RING_CASES, ids=lambda j: j["id"])
 def test_ring_window_within_model(runs, job):
-    rb.check_window_case(job, rh.load_ring_case(job, runs.outdir(job["world"])))
+    rh.check_ring_case(job, rh.load_ring_case(job, runs.outdir(job["world"])))
 
 
 def test_report_worst_ratios():

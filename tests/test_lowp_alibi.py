@@ -21,10 +21,10 @@ MUTANT_CASES = la.MUTANT_CASES
 
 def run_case(case, mutant=None, device="cpu"):
     x = la.make_alibi_inputs(case, device)
-    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], x["alibis"])
-    got = la.lowp_alibi_chain(*args, mutant=mutant)
-    ref = la.oracle_alibi_chain(*args)
-    model = got if mutant is None else la.lowp_alibi_chain(*args)
+    args = (x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"])
+    got = lm.lowp_chain(*args, mutant=mutant, alibis=x["alibis"])
+    ref = lm.oracle_chain(*args, alibis=x["alibis"])
+    model = got if mutant is None else lm.lowp_chain(*args, alibis=x["alibis"])
     absmax = la.absmax_prefix(x["q"], x["ks"], x["scale"], x["masks"], x["alibis"])
     lm.assert_chain_within_model(case["id"], got, ref, model, case["dtype"], absmax)
 
@@ -64,7 +64,7 @@ def test_sweep_covers_every_alibi_edge():
     for c in la.ALIBI_SWEEP:
         if len(c["chunks"]) > 1:
             x = la.make_alibi_inputs(c)
-            la.lowp_alibi_chain(x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], x["alibis"], info=info)
+            lm.lowp_chain(x["q"], x["ks"], x["vs"], x["do"], x["scale"], x["masks"], alibis=x["alibis"], info=info)
     assert info.get("lowered", 0) > 0 and info.get("kept", 0) > 0, info
     # the far cases: beyond 2^24 (the loader's fp32 row term inexact), and far chains at slopes of 0.5 and more
     assert any(abs(d) > 2 ** 24 for c in la.ALIBI_SWEEP for d in c["dist0s"])

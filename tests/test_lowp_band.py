@@ -14,8 +14,6 @@ import torch
 import lowp_band as lb
 import lowp_model as lm
 
-lb.install()
-
 _BY_ID = {c["id"]: c for c in lb.BAND_SWEEP}
 BF16, FP16 = torch.bfloat16, torch.float16
 MUTANT_CASES = lb.MUTANT_CASES

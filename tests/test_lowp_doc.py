@@ -14,8 +14,6 @@ import torch
 import lowp_doc as ld
 import lowp_model as lm
 
-ld.install()
-
 BF16, FP16 = torch.bfloat16, torch.float16
 MUTANT_CASES = ld.mutant_cases()
 

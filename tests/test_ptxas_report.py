@@ -3,7 +3,8 @@
 ptxas serializes a kernel's whole wgmma pipeline (waits after every MMA) when the kernel makes a function call, e.g.
 a printf, or when a wgmma group crosses a divergent path; it says so in an info line ("C7510" / "C7520 Potential
 Performance Loss").  A spill puts local-memory traffic in the inner loop.  Both are silent slowdowns, so every
-instantiation of fwd_chunk_kernel and bwd_chunk_kernel is checked here with the flags of csrc/Makefile.
+instantiation of the tile kernels -- plain, band, ALiBi and packed-document -- is checked here with the flags of
+csrc/Makefile.
 """
 import os
 import re
@@ -52,7 +53,13 @@ def _per_kernel(log, kernel):
 
 
 @pytest.mark.parametrize("src,kernel,n_inst", [("fwd_sm90.cu", "fwd_chunk_kernel", 8),
-                                               ("bwd_sm90.cu", "bwd_chunk_kernel", 4)])
+                                               ("bwd_sm90.cu", "bwd_chunk_kernel", 4),
+                                               ("fwd_band_sm90.cu", "fwd_chunk_kernel", 8),
+                                               ("bwd_band_sm90.cu", "bwd_chunk_kernel", 4),
+                                               ("fwd_alibi_sm90.cu", "fwd_alibi_kernel", 8),
+                                               ("bwd_alibi_sm90.cu", "bwd_alibi_kernel", 8),
+                                               ("fwd_doc_sm90.cu", "fwd_doc_kernel", 4),
+                                               ("bwd_doc_sm90.cu", "bwd_doc_kernel", 4)])
 def test_tile_kernels_not_serialized_and_no_spills(src, kernel, n_inst, tmp_path):
     log = _ptxas_report(src, tmp_path)
     assert "C7510" not in log and "Performance Loss" not in log, \

@@ -1,5 +1,5 @@
 """Packed documents (cu_seqlens) without a GPU: the document oracle, the ring drivers under gloo with the fp64 oracle
-chunk operators (doc_ops), the planner's launches per round, the doc kernels' index arithmetic restated in Python
+chunk operators (oracle_ops), the planner's launches per round, the doc kernels' index arithmetic restated in Python
 (doc_index: the deterministic-mode deadlock precondition), and argument checks of the public API and of the C-ABI."""
 import ctypes
 import os
@@ -8,9 +8,8 @@ import pytest
 import torch
 import torch.distributed as dist
 
-import band_oracle as bo
 import doc_index as di
-import doc_oracle
+import mask_oracle as mo
 from ring_harness import double_group, spawn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,7 +27,7 @@ def test_doc_oracle_matches_double_loop():
     S, cu = 11, [0, 3, 3, 7, 11]
     q, k, v = (torch.randn(1, S, 2, 4, dtype=torch.float64) for _ in range(3))
     for causal, window in ((False, None), (True, None), (True, (2, -1)), (False, (1, 2))):
-        o, lse, *_ = doc_oracle.dense_attention_bwd(q, k, v, torch.zeros_like(q), cu, 0.5, causal, window)
+        o, lse, *_ = mo.dense_attention_bwd(q, k, v, torch.zeros_like(q), 0.5, causal, window, cu=cu)
         for a in range(S):
             d = max(i for i in range(len(cu) - 1) if cu[i] <= a)
             js = [c for c in range(cu[d], cu[d + 1]) if (not causal or c <= a) and
@@ -38,8 +37,8 @@ def test_doc_oracle_matches_double_loop():
             torch.testing.assert_close(o[0, a], torch.einsum("nh,nhd->hd", torch.softmax(s, 0), v[0, js]))
             torch.testing.assert_close(lse[0, :, a], torch.logsumexp(s, 0))
     # one document is the plain windowed oracle
-    o1 = doc_oracle.dense_attention_bwd(q, k, v, q, [0, S], 0.5, True, (3, -1))
-    o2 = bo.dense_attention_bwd(q, k, v, q, 0.5, True, (3, -1))
+    o1 = mo.dense_attention_bwd(q, k, v, q, 0.5, True, (3, -1), cu=[0, S])
+    o2 = mo.dense_attention_bwd(q, k, v, q, 0.5, True, (3, -1))
     for a, b in zip(o1, o2):
         torch.testing.assert_close(a, b)
 
@@ -55,9 +54,8 @@ def _check(rank, world, layout, cu, window=(-1, -1), causal=None, dg=(None, None
     q, do = (torch.randn(B, S, H, D, dtype=torch.float64) for _ in range(2))
     k, v = (torch.randn(B, S, Hkv, D, dtype=torch.float64) for _ in range(2))
     G = H // Hkv
-    o_ref, _, dq_ref, dk_ref, dv_ref = doc_oracle.dense_attention_bwd(q, k.repeat_interleave(G, 2),
-                                                                      v.repeat_interleave(G, 2), do, cu, 0.3, causal,
-                                                                      window)
+    o_ref, _, dq_ref, dk_ref, dv_ref = mo.dense_attention_bwd(q, k.repeat_interleave(G, 2), v.repeat_interleave(G, 2),
+                                                              do, 0.3, causal, window, cu=cu)
     dk_ref, dv_ref = (t.unflatten(2, (Hkv, G)).sum(3) for t in (dk_ref, dv_ref))
     lay = (lambda t: t) if seq_dim == 1 else (lambda t: t.permute(0, 2, 1, 3).contiguous())
     sh = lambda t: lay(orc.shard(t, rank, world, layout))  # noqa: E731
@@ -72,7 +70,9 @@ def _check(rank, world, layout, cu, window=(-1, -1), causal=None, dg=(None, None
         torch.testing.assert_close(got, sh(ref), **TOL)
     # the forward's launches attend exactly this rank's visible (query, key) position pairs, each once
     pos = orc.shard(torch.arange(S).view(1, S, 1, 1), rank, world, layout).view(-1).tolist()
-    vis = doc_oracle.visible(S, cu, causal, window)
+    vis = mo.same_doc(torch.arange(S), torch.arange(S), cu)
+    w = mo.window_mask(S, S, window, causal)
+    vis = vis if w is None else vis & w
     want = {(a, c) for a in pos for c in vis[a].nonzero().view(-1).tolist()}
     assert ops.pairs == want
 
@@ -80,8 +80,8 @@ def _check(rank, world, layout, cu, window=(-1, -1), causal=None, dg=(None, None
 def _worker(rank, world, port, intra):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from burst_attn import chunk_ops
-    from doc_ops import DocOracleOps
-    chunk_ops._set_ops_for_testing(DocOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         dg = double_group(rank, world, intra, False) if intra else (None, None)
         S = 12 * world
@@ -110,10 +110,10 @@ def test_doc_ring_matches_dense(world, intra):
 @pytest.mark.parametrize("blk", [None, "16"])
 def test_doc_world1_and_l2_blocks(monkeypatch, blk):
     from burst_attn import chunk_ops
-    from doc_ops import DocOracleOps
+    from oracle_ops import OracleOps
     if blk:
         monkeypatch.setenv("BA_L2_BLOCK", blk)
-    chunk_ops._set_ops_for_testing(DocOracleOps())
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         for layout in ("contiguous", "zigzag", "striped"):
             for cu in _cus(70):
@@ -127,10 +127,10 @@ def test_doc_world1_and_l2_blocks(monkeypatch, blk):
 def test_flash_attn_varlen_func_cpu(monkeypatch, blk):
     from burst_attn import chunk_ops
     from burst_attn.flash_triton import flash_attn_varlen_func
-    from doc_ops import DocOracleOps
+    from oracle_ops import OracleOps
     if blk:
         monkeypatch.setenv("BA_L2_BLOCK", blk)
-    chunk_ops._set_ops_for_testing(DocOracleOps())
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         torch.manual_seed(4)
         T = 90
@@ -144,9 +144,9 @@ def test_flash_attn_varlen_func_cpu(monkeypatch, blk):
                 qq, kk, vv = (t.clone().requires_grad_() for t in (q, k, v))
                 o = flash_attn_varlen_func(qq, kk, vv, cut, cut, longest, longest, 0.0, 0.25, causal, window)
                 g = torch.autograd.grad(o, (qq, kk, vv), do)
-                o_r, _, dq, dk, dv = doc_oracle.dense_attention_bwd(q[None], k[None].repeat_interleave(2, 2),
-                                                                    v[None].repeat_interleave(2, 2), do[None], cu,
-                                                                    0.25, causal, window)
+                o_r, _, dq, dk, dv = mo.dense_attention_bwd(q[None], k[None].repeat_interleave(2, 2),
+                                                            v[None].repeat_interleave(2, 2), do[None], 0.25, causal,
+                                                            window, cu=cu)
                 torch.testing.assert_close(o.detach(), o_r[0], **TOL)
                 torch.testing.assert_close(g[0], dq[0], **TOL)
                 torch.testing.assert_close(g[1], dk[0].unflatten(1, (2, 2)).sum(2), **TOL)
@@ -159,8 +159,8 @@ def _calls_worker(rank, world, port, outdir):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from burst_attn import burst_attn_func, burst_attn_func_striped, chunk_ops
     from oracle import attention_oracle as orc
-    from doc_ops import DocOracleOps
-    ops = DocOracleOps()
+    from oracle_ops import OracleOps
+    ops = OracleOps()
     chunk_ops._set_ops_for_testing(ops)
     try:
         S_local = 8
@@ -194,7 +194,7 @@ def test_rounds_without_a_shared_document_launch_nothing(tmp_path):
     world = 4
     spawn(_calls_worker, world, (str(tmp_path),), timeout=300)
     for rank in range(world):
-        res = torch.load(os.path.join(tmp_path, f"calls{rank}.pt"))
+        res = torch.load(os.path.join(tmp_path, f"calls{rank}.pt"), weights_only=False)  # oracle_ops.Call records
         calls = res[("contiguous", "inside")]
         fwd = [c for c in calls if c[0] == "fwd"]
         bwd = [c for c in calls if c[0] == "bwd"]
@@ -261,8 +261,8 @@ def test_index_check_rejects_mutants(mutant):
 def test_bad_cu_seqlens_raise(bad, err, match):
     from burst_attn import burst_attn_func, burst_attn_func_striped, chunk_ops
     from burst_attn.flash_triton import flash_attn_varlen_func
-    from doc_ops import DocOracleOps
-    chunk_ops._set_ops_for_testing(DocOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         q = torch.randn(1, 24, 2, 8, dtype=torch.float64)
         cu = {"int64": torch.tensor([0, 24]), "list": [0, 24]}.get(bad) if isinstance(bad, str) else \
@@ -279,8 +279,8 @@ def test_bad_cu_seqlens_raise(bad, err, match):
 def test_unsupported_combinations_raise():
     from burst_attn import burst_attn_func, chunk_ops
     from burst_attn.flash_triton import flash_attn_varlen_func
-    from doc_ops import DocOracleOps
-    chunk_ops._set_ops_for_testing(DocOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         q = torch.randn(24, 2, 8, dtype=torch.float64)
         cu = torch.tensor([0, 10, 24], dtype=torch.int32)

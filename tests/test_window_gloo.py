@@ -8,7 +8,7 @@ import pytest
 import torch
 import torch.distributed as dist
 
-import band_oracle as bo
+import mask_oracle as mo
 from ring_harness import double_group, spawn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -21,7 +21,7 @@ def test_window_mask_matches_double_loop():
     for sq, sk in [(7, 7), (5, 11), (9, 4)]:
         for causal in (False, True):
             for left, right in WINDOWS + [(-1, -1), (2, 0), (30, 30)]:
-                m = bo.window_mask(sq, sk, (left, right), causal)
+                m = mo.window_mask(sq, sk, (left, right), causal)
                 r = 0 if causal else right
                 for i in range(sq):
                     for j in range(sk):
@@ -34,7 +34,7 @@ def test_windowed_oracle_matches_double_loop_and_causal():
     from oracle import attention_oracle as orc
     torch.manual_seed(3)
     q, k, v = (torch.randn(1, n, 2, 8, dtype=torch.float64) for n in (6, 9, 9))
-    o, lse = bo.dense_attention(q, k, v, 0.5, False, (2, 1))
+    o, lse = mo.dense_attention(q, k, v, 0.5, False, (2, 1))
     for i in range(6):
         p = i + 3
         js = [j for j in range(9) if p - 2 <= j <= p + 1]
@@ -42,12 +42,12 @@ def test_windowed_oracle_matches_double_loop_and_causal():
         w = torch.softmax(s, 0)
         torch.testing.assert_close(o[0, i], torch.einsum("nh,nhd->hd", w, v[0, js]))
         torch.testing.assert_close(lse[0, :, i], torch.logsumexp(s, 0))
-    o1, l1 = bo.dense_attention(q, k, v, 0.5, False, (-1, 0))
+    o1, l1 = mo.dense_attention(q, k, v, 0.5, False, (-1, 0))
     o2, l2 = orc.dense_attention(q, k, v, 0.5, True)
     torch.testing.assert_close(o1, o2)
     torch.testing.assert_close(l1, l2)
     do = torch.randn_like(q)
-    for a, b in zip(bo.dense_attention_bwd(q, k, v, do, 0.5, True, (-1, -1)), orc.dense_attention_bwd(q, k, v, do, 0.5, True)):
+    for a, b in zip(mo.dense_attention_bwd(q, k, v, do, 0.5, True, (-1, -1)), orc.dense_attention_bwd(q, k, v, do, 0.5, True)):
         torch.testing.assert_close(a, b)
 
 
@@ -60,7 +60,7 @@ def _check(ops, rank, world, layout, window, dg=(None, None), S_local=12):
     torch.manual_seed(77)
     B, S, H, D = 1, S_local * world, 2, 8
     q, k, v, do = (torch.randn(B, S, H, D, dtype=torch.float64) for _ in range(4))
-    o_ref, _, dq_ref, dk_ref, dv_ref = bo.dense_attention_bwd(q, k, v, do, 0.3, causal, window)
+    o_ref, _, dq_ref, dk_ref, dv_ref = mo.dense_attention_bwd(q, k, v, do, 0.3, causal, window)
     sh = lambda t: orc.shard(t, rank, world, shard)  # noqa: E731
     ql, kl, vl = (sh(t).requires_grad_() for t in (q, k, v))
     o = func(ql, kl, vl, 0.3, "cuda", causal, False, False, None, list(dg), window)
@@ -74,8 +74,8 @@ def _check(ops, rank, world, layout, window, dg=(None, None), S_local=12):
 def _worker(rank, world, port, intra):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from burst_attn import chunk_ops
-    from band_ops import BandOracleOps
-    chunk_ops._set_ops_for_testing(BandOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         dg = double_group(rank, world, intra, False) if intra else (None, None)
         for layout in ("contiguous", "zigzag", "striped", "striped_nc"):
@@ -98,8 +98,8 @@ def test_windowed_world1_and_l2_blocks(monkeypatch):
     """One rank, with and without L2 blocking of the rounds (BA_L2_BLOCK = 16: rows whose first visible key block is
     not block 0, and rows the last launch does not visit)."""
     from burst_attn import chunk_ops
-    from band_ops import BandOracleOps
-    chunk_ops._set_ops_for_testing(BandOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         for blk in (None, "16"):
             if blk:
@@ -115,10 +115,10 @@ def test_windowed_world1_and_l2_blocks(monkeypatch):
 def test_flash_wrappers_window_cpu(monkeypatch, blk):
     from burst_attn import chunk_ops
     from burst_attn.flash_triton import flash_attn_func, flash_attn_kvpacked_func, flash_attn_qkvpacked_func
-    from band_ops import BandOracleOps
+    from oracle_ops import OracleOps
     if blk:
         monkeypatch.setenv("BA_L2_BLOCK", blk)
-    chunk_ops._set_ops_for_testing(BandOracleOps())
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         torch.manual_seed(9)
         for sq, sk in [(70, 70), (50, 110), (110, 45)]:
@@ -130,7 +130,7 @@ def test_flash_wrappers_window_cpu(monkeypatch, blk):
                     o = flash_attn_func(qq, kk, vv, None, causal, 0.25, window)
                     g = torch.autograd.grad(o, (qq, kk, vv), do)
                     ke, ve = k.repeat_interleave(2, 2), v.repeat_interleave(2, 2)
-                    o_ref, _, dq, dk, dv = bo.dense_attention_bwd(q, ke, ve, do, 0.25, causal, window)
+                    o_ref, _, dq, dk, dv = mo.dense_attention_bwd(q, ke, ve, do, 0.25, causal, window)
                     tol = dict(rtol=1e-5, atol=1e-5)  # fp32 accumulators in the driver
                     torch.testing.assert_close(o.detach(), o_ref, **tol)
                     torch.testing.assert_close(g[0], dq, **tol)
@@ -142,7 +142,7 @@ def test_flash_wrappers_window_cpu(monkeypatch, blk):
             if sq == sk:
                 qkv = torch.stack([q, q, q], 2).requires_grad_()
                 o3 = flash_attn_qkvpacked_func(qkv, None, True, 0.25, (9, -1))
-                torch.testing.assert_close(o3.detach(), bo.dense_attention(q, q, q, 0.25, True, (9, -1))[0], rtol=1e-5,
+                torch.testing.assert_close(o3.detach(), mo.dense_attention(q, q, q, 0.25, True, (9, -1))[0], rtol=1e-5,
                                            atol=1e-5)
     finally:
         chunk_ops._set_ops_for_testing(None)
@@ -152,8 +152,8 @@ def _calls_worker(rank, world, port, outdir):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from burst_attn import burst_attn_func, burst_attn_func_striped, chunk_ops
     from oracle import attention_oracle as orc
-    from band_ops import BandOracleOps
-    ops = BandOracleOps()
+    from oracle_ops import OracleOps
+    ops = OracleOps()
     chunk_ops._set_ops_for_testing(ops)
     try:
         S_local = 8
@@ -183,7 +183,7 @@ def test_rounds_outside_the_window_launch_nothing(tmp_path):
     world, S = 8, 8
     spawn(_calls_worker, world, (str(tmp_path),), timeout=300)
     for rank in range(world):
-        res = torch.load(os.path.join(tmp_path, f"calls{rank}.pt"))
+        res = torch.load(os.path.join(tmp_path, f"calls{rank}.pt"), weights_only=False)  # oracle_ops.Call records
         for name in ("contiguous", "zigzag", "striped"):
             assert res[(name, "omitted")] == res[(name, "minus1")], name
         calls = res[("contiguous", "half")]
@@ -194,7 +194,7 @@ def test_rounds_outside_the_window_launch_nothing(tmp_path):
         for c in fwd + bwd:
             assert c[1][1] == S and c[2][1] == S  # whole shards: no L2 split at this size
         # the own shard: the window's two sides; the neighbours: one side each (the other masks nothing)
-        assert sorted((c[3], c[4], c[-1]) for c in fwd) == sorted(
+        assert sorted((c.causal, c.causal_offset, c.lower) for c in fwd) == sorted(
             [(True, S // 2, -S // 2)] + ([(False, 0, S // 2)] if rank > 0 else []) +
             ([(True, -S // 2, None)] if rank < world - 1 else []))
 
@@ -203,8 +203,8 @@ def test_rounds_outside_the_window_launch_nothing(tmp_path):
 def test_bad_window_raises(window):
     from burst_attn import burst_attn_func, chunk_ops
     from burst_attn.flash_triton import flash_attn_func
-    from band_ops import BandOracleOps
-    chunk_ops._set_ops_for_testing(BandOracleOps())
+    from oracle_ops import OracleOps
+    chunk_ops._set_ops_for_testing(OracleOps())
     try:
         q = torch.randn(1, 8, 1, 8, dtype=torch.float64)
         with pytest.raises(ValueError, match="window_size"):
@@ -262,7 +262,6 @@ def test_band_mutants_rejected_by_the_model_cpu():
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import lowp_band
     import lowp_model as lm
-    lowp_band.install()
     case = lm._case(257, [(257, None)], 64, torch.bfloat16, tag="band_mutant_cpu_")
     x = lm.make_inputs(case)
     x["masks"] = [("band", -70, 10)]
@@ -270,9 +269,9 @@ def test_band_mutants_rejected_by_the_model_cpu():
     model, ref = lm.lowp_chain(*args), lm.oracle_chain(*args)
     absmax = [lm.scores_absmax(x["q"], x["ks"], x["scale"], x["masks"])]
     lm.assert_chain_within_model("band", model, ref, model, torch.bfloat16, absmax)
-    vis = lowp_band.visible(257, 257, x["masks"][0])
+    vis = lm.visible(257, 257, x["masks"][0])
     live = [m for m in lowp_band.BAND_MUTANTS
-            if any(not torch.equal(lowp_band.vis_for(257, 257, x["masks"][0], None, m, side), vis)
+            if any(not torch.equal(lm._vis_for(257, 257, x["masks"][0], None, m, side), vis)
                    for side in ("fwd", "bwd"))]
     assert {"band_lo_plus1_fwd", "band_lo_plus1_bwd", "band_i_end_short"} <= set(live), live
     for mutant in live:
