@@ -122,7 +122,7 @@ def chunk_forward(q, k, v, o_acc, lse, scale, mask_mode="none", dtype=torch.floa
     s = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale
     if key_bias is not None:  # [B|1,H,Sk] additive bias per key (the LAO tile's "vector" bias, lao.py:155-173)
         s = s + key_bias.to(dtype).unsqueeze(2)
-    m = _mask(s.shape[-2], s.shape[-1], mask_mode)
+    m = _mask(s.shape[-2], s.shape[-1], mask_mode, s.device)
     if m is not None:
         s = s.masked_fill(~m, NEG_INF)
     lse_i = torch.logsumexp(s, dim=-1)  # [B,H,Sq]; -inf where nothing visible
@@ -163,7 +163,7 @@ def chunk_backward(do, q, k, v, delta, lse, scale, mask_mode="none", dtype=torch
     if key_bias is not None:
         s = s + key_bias.to(dtype).unsqueeze(2)
     p = torch.exp(s - lse.unsqueeze(-1))
-    m = _mask(s.shape[-2], s.shape[-1], mask_mode)
+    m = _mask(s.shape[-2], s.shape[-1], mask_mode, s.device)
     if m is not None:
         p = p.masked_fill(~m, 0.0)
     dv = torch.einsum("bhqk,bqhd->bkhd", p, do)

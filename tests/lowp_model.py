@@ -584,18 +584,18 @@ def lowp_chain(q, ks, vs, do, scale, masks, biases=None, mutant=None, alibis=Non
     return dict(o=o, lse=lse, states=states, dq=dq, dk=dks, dv=dvs)
 
 
-def oracle_chain(q, ks, vs, do, scale, masks, biases=None, alibis=None):
-    """The same chain in fp64 with ``mask_oracle`` (on the CPU), on the same 16-bit inputs; ALiBi enters as each
-    chunk's pair bias (``mask_oracle.chunk_bias``)."""
+def oracle_chain(q, ks, vs, do, scale, masks, biases=None, alibis=None, device="cpu"):
+    """The same chain in fp64 with ``mask_oracle`` (on ``device``, the CPU by default), on the same 16-bit inputs;
+    ALiBi enters as each chunk's pair bias (``mask_oracle.chunk_bias``)."""
     n = len(ks)
-    cpu = lambda t: None if t is None else t.detach().cpu()  # noqa: E731
-    q, do = cpu(q), cpu(do)
+    dev = lambda t: None if t is None else t.detach().to(device)  # noqa: E731
+    q, do = dev(q), dev(do)
     H, Hkv = q.shape[2], ks[0].shape[2]
-    kx = [_kv_heads(cpu(k), H) for k in ks]
-    vx = [_kv_heads(cpu(v), H) for v in vs]
-    biases = [cpu(b) for b in biases] if biases else [None] * n
+    kx = [_kv_heads(dev(k), H) for k in ks]
+    vx = [_kv_heads(dev(v), H) for v in vs]
+    biases = [dev(b) for b in biases] if biases else [None] * n
     if alibis:
-        biases = [b if a is None else mo.chunk_bias((cpu(a[0]), a[1], a[2]), q.shape[1], kx[c].shape[1])
+        biases = [b if a is None else mo.chunk_bias((dev(a[0]), a[1], a[2]), q.shape[1], kx[c].shape[1])
                   for c, (a, b) in enumerate(zip(alibis, biases))]
     o, lse, states = None, None, []
     for c in range(n):
@@ -604,7 +604,7 @@ def oracle_chain(q, ks, vs, do, scale, masks, biases=None, alibis=None):
             states.append((o, lse))
     delta = orc.compute_delta(o, do)
     lse_b = torch.where(torch.isinf(lse), torch.full_like(lse, float("inf")), lse)  # dead rows: P = 0
-    dq = torch.zeros(q.shape, dtype=torch.float64)
+    dq = torch.zeros(q.shape, dtype=torch.float64, device=q.device)
     dks, dvs = [], []
     for c in range(n):
         dqc, dk, dv = mo.chunk_backward(do, q, kx[c], vx[c], delta, lse_b, scale, masks[c], bias=biases[c])
@@ -616,9 +616,18 @@ def oracle_chain(q, ks, vs, do, scale, masks, biases=None, alibis=None):
 
 
 def error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, biases, Hkv):
-    """The comparator's error scales of one fp64 chain (``oracle_chain``): dict(mag, rss, e32).  CPU tensors; kx / vx
-    per chunk at the query heads; lse_b the final lse with +inf for dead rows; ``biases[c]``: None, a key bias
-    [B|1,H,Sk] or a pair bias [B,H,Sq,Sk], in natural units."""
+    """The comparator's error scales of one fp64 chain (``oracle_chain``): dict(mag, rss, e32, sums).  Tensors on one
+    device; kx / vx per chunk at the query heads; lse_b the final lse with +inf for dead rows; ``biases[c]``: None, a
+    key bias [B|1,H,Sk] or a pair bias [B,H,Sq,Sk], in natural units.  ``sums``: the ``error_sums`` the scales are
+    finished from (``finish_scales``)."""
+    sums = error_sums(q, kx, vx, do, o, delta, lse_b, scale, masks, biases)
+    return dict(mag=magnitudes(q, kx, vx, do, scale), sums=sums,
+                **finish_scales(sums, o, Hkv, [k.shape[1] for k in kx]))
+
+
+def error_sums(q, kx, vx, do, o, delta, lse_b, scale, masks, biases):
+    """The additive parts of ``error_scales``: per row (fp64 [B,Sq,H]) and, per chunk, per key and query head (fp64
+    [B,Sk,H]) sums over the pairs a chain sees.  A problem cut into row blocks adds the per-key sums of its blocks."""
     n = len(kx)
     # Per gradient row, two error scales no 16-bit model run reproduces by itself:
     # rss: the root sum of squares of the row's terms (P V for O, P dO for dV, dS K scale for dQ, dS Q scale for dK).
@@ -626,16 +635,14 @@ def error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, biases, Hkv):
     #   exactly) or one term dominates, one model run can happen to land near the truth while the kernel does not.
     #   delta comes from the 16-bit O, whose rounding moves delta by ~u sqrt(sum_d (O_d dO_d)^2) and every dS of the
     #   row by P times that: in a peaky row this term, not the rounding of dS, dominates dQ and dK (for dK the
-    #   rows' shifts are added coherently, an upper bound).
+    #   rows' shifts are added coherently, an upper bound: ``dk_coh`` is that sum, squared in ``finish_scales``).
     # e32: dS = P (dP - delta) with dP from fp32 tensor-core accumulation and delta from a separate fp32 sum keeps
     #   ~2^-23 sum_d |dO_d V_d| of rounding per element, which reaches dQ through |K| and dK through |Q|.
-    ss = dict(o=torch.zeros(q.shape[:3], dtype=torch.float64), dq=torch.zeros(q.shape[:3], dtype=torch.float64))
-    ss_dk, ss_dv, e32_dk = [], [], []
-    e32_dq = torch.zeros(q.shape[:3], dtype=torch.float64)
+    z = lambda: torch.zeros(q.shape[:3], dtype=torch.float64, device=q.device)  # noqa: E731
+    out = dict(o=z(), dq=z(), dq_coh=z(), e32_dq=z(), dk=[], dk_coh=[], dv=[], e32_dk=[])
     qd, dod = q.double(), do.double()
     n2 = lambda t: t.double().pow(2).sum(-1)  # noqa: E731  [B,S,H] squared row norms
     dd = n2(o.double() * dod).sqrt().permute(0, 2, 1)  # [B,H,Sq]
-    dq_d = torch.zeros(q.shape[:3], dtype=torch.float64)
     for c in range(n):
         kd, vd = kx[c].double(), vx[c].double()
         s = torch.einsum("bqhd,bkhd->bhqk", qd, kd) * scale
@@ -643,51 +650,65 @@ def error_scales(q, kx, vx, do, o, delta, lse_b, scale, masks, biases, Hkv):
             b = biases[c].double()
             s = s + (b if b.dim() == 4 else b.unsqueeze(2))
         p = torch.exp(s - lse_b.unsqueeze(-1))
-        vis = visible(q.shape[1], kd.shape[1], masks[c])
+        del s
+        vis = visible(q.shape[1], kd.shape[1], masks[c], q.device)
         if vis is not None:
             p = p.masked_fill(~vis, 0.0)
         ds = p * (torch.einsum("bqhd,bkhd->bhqk", dod, vd) - delta.unsqueeze(-1)) * scale
-        ss["o"] += torch.einsum("bhqk,bkh->bqh", p * p, n2(vd))
+        out["o"] += torch.einsum("bhqk,bkh->bqh", p * p, n2(vd))
         pd = p * dd.unsqueeze(-1) * abs(scale)  # [B,H,Sq,Sk]: the dS shift of one unit of delta rounding
-        ss["dq"] += torch.einsum("bhqk,bkh->bqh", ds * ds, n2(kd))
-        dq_d = dq_d + torch.einsum("bhqk,bkh->bqh", pd, kd.norm(dim=-1))
-        ss_dk.append(_group_sum((torch.einsum("bhqk,bqh->bkh", ds * ds, n2(qd)) +
-                                 torch.einsum("bhqk,bqh->bkh", pd, qd.norm(dim=-1)).pow(2)).unsqueeze(-1), Hkv)[..., 0])
-        ss_dv.append(_group_sum(torch.einsum("bhqk,bqh->bkh", p * p, n2(dod)).unsqueeze(-1), Hkv)[..., 0])
+        out["dq"] += torch.einsum("bhqk,bkh->bqh", ds * ds, n2(kd))
+        out["dq_coh"] += torch.einsum("bhqk,bkh->bqh", pd, kd.norm(dim=-1))
+        out["dk"].append(torch.einsum("bhqk,bqh->bkh", ds * ds, n2(qd)))
+        out["dk_coh"].append(torch.einsum("bhqk,bqh->bkh", pd, qd.norm(dim=-1)))
+        out["dv"].append(torch.einsum("bhqk,bqh->bkh", p * p, n2(dod)))
+        del ds, pd
         w = 2.0 ** -23 * abs(scale) * p * torch.einsum("bqhd,bkhd->bhqk", dod.abs(), vd.abs())
-        e32_dq += torch.einsum("bhqk,bkh->bqh", w, kd.norm(dim=-1))
-        e32_dk.append(_group_sum(torch.einsum("bhqk,bqh->bkh", w, qd.norm(dim=-1)).unsqueeze(-1), Hkv)[..., 0])
-    rss = dict(o=(ss["o"] + n2(o)).sqrt(), dq=(ss["dq"] + dq_d.pow(2)).sqrt(), dk=torch.cat(ss_dk, 1).sqrt(),
-               dv=torch.cat(ss_dv, 1).sqrt())
-    # the size of one key's contribution to a gradient row, before any cancellation (the comparator's floor)
+        out["e32_dq"] += torch.einsum("bhqk,bkh->bqh", w, kd.norm(dim=-1))
+        out["e32_dk"].append(torch.einsum("bhqk,bqh->bkh", w, qd.norm(dim=-1)))
+    return out
+
+
+def finish_scales(sums, o, Hkv, sks):
+    """dict(rss, e32) of ``error_sums`` (dK / dV per key, the chunks' keys in order, their K/V heads summed)."""
+    n2 = lambda t: t.double().pow(2).sum(-1)  # noqa: E731
+    g = lambda t: _group_sum(t.unsqueeze(-1), Hkv)[..., 0]  # noqa: E731  [B,Sk,H] -> [B,Sk,Hkv]
+    rss = dict(o=(sums["o"] + n2(o)).sqrt(), dq=(sums["dq"] + sums["dq_coh"].pow(2)).sqrt(),
+               dk=torch.cat([g(a + c.pow(2)) for a, c in zip(sums["dk"], sums["dk_coh"])], 1).sqrt(),
+               dv=torch.cat([g(a) for a in sums["dv"]], 1).sqrt())
+    return dict(rss=rss, e32=dict(dq=sums["e32_dq"], dk=torch.cat([g(a) for a in sums["e32_dk"]], 1)))
+
+
+def magnitudes(q, kx, vx, do, scale):
+    """The size of one key's contribution to a gradient row, before any cancellation (the comparator's floor):
+    dict(dq, dk, dv) from the largest row norms of the inputs (kx / vx: the chunks' K / V)."""
     nrm = lambda ts: max(float(t.double().norm(dim=-1).max()) for t in ts)  # noqa: E731
     nq, ndo, nk, nv = nrm([q]), nrm([do]), nrm(kx), nrm(vx)
-    mag = dict(dq=abs(scale) * ndo * nv * nk, dk=abs(scale) * ndo * nv * nq, dv=ndo)
-    return dict(mag=mag, rss=rss, e32=dict(dq=e32_dq, dk=torch.cat(e32_dk, 1)))
+    return dict(dq=abs(scale) * ndo * nv * nk, dk=abs(scale) * ndo * nv * nq, dv=ndo)
 
 
-def scores_absmax(q, ks, scale, masks, biases=None):
+def scores_absmax(q, ks, scale, masks, biases=None, device="cpu"):
     """[B,H,Sq]: per row, the largest ``sum_d |q_d k_d| scale + |bias|`` over the keys the row sees in any chunk --
     the magnitude the fp32 score arithmetic works at, which bounds its rounding error.  ``biases[c]``: None, a key
-    bias [B|1,H,Sk] or a pair bias [B,H,Sq,Sk]."""
+    bias [B|1,H,Sk] or a pair bias [B,H,Sq,Sk].  Computed on ``device``."""
     n = len(ks)
     biases = biases or [None] * n
-    q = q.detach().cpu().double().abs()
+    q = q.detach().to(device).double().abs()
     H = q.shape[2]
-    out = torch.zeros(q.shape[0], H, q.shape[1], dtype=torch.float64)
+    out = torch.zeros(q.shape[0], H, q.shape[1], dtype=torch.float64, device=q.device)
     for c in range(n):
-        k = _kv_heads(ks[c].detach().cpu(), H).double().abs()
+        k = _kv_heads(ks[c].detach().to(device), H).double().abs()
         a = torch.einsum("bqhd,bkhd->bhqk", q, k) * abs(scale)
         pair = biases[c] is not None and biases[c].dim() == 4
         if biases[c] is not None:
-            bb = biases[c].detach().cpu().double().abs()
+            bb = biases[c].detach().to(device).double().abs()
             bb = torch.where(torch.isinf(bb), torch.zeros_like(bb), bb)
             a = a + (bb if pair else bb.unsqueeze(2))
-        vis = visible(q.shape[1], k.shape[1], masks[c])
+        vis = visible(q.shape[1], k.shape[1], masks[c], q.device)
         if vis is not None:
             a = a.masked_fill(~vis, 0.0)
         if biases[c] is not None:
-            inf = torch.isinf(biases[c].detach().cpu())
+            inf = torch.isinf(biases[c].detach().to(device))
             a = a.masked_fill((inf if pair else inf.unsqueeze(2)).expand_as(a), 0.0)
         out = torch.maximum(out, a.amax(-1))
     return out

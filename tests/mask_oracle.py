@@ -36,24 +36,24 @@ def same_doc(pos_q, pos_k, cu):
     return doc_ids(pos_q, cu).unsqueeze(1) == doc_ids(pos_k, cu).unsqueeze(0)
 
 
-def mask_of(sq, sk, mask):
-    """[sq, sk] bool of a kernel mask (see the module docstring), or None when nothing is masked."""
+def mask_of(sq, sk, mask, device=None):
+    """[sq, sk] bool of a kernel mask (see the module docstring) on ``device``, or None when nothing is masked."""
     if mask is None or mask == "none":
         return None
-    a = torch.arange(sq).unsqueeze(1)
-    b = torch.arange(sk).unsqueeze(0)
+    a = torch.arange(sq, device=device).unsqueeze(1)
+    b = torch.arange(sk, device=device).unsqueeze(0)
     if mask[0] == "causal_offset":
         return b <= a + int(mask[1])
     assert mask[0] in ("band", "doc"), mask
     lo, hi = mask[1], mask[2]
-    m = torch.ones(sq, sk, dtype=torch.bool)
+    m = torch.ones(sq, sk, dtype=torch.bool, device=device)
     if lo is not None:
         m &= b >= a + int(lo)
     if hi is not None:
         m &= b <= a + int(hi)
     if mask[0] == "doc":
         _, _, _, cu, q_pos0, k_pos0, ps = mask
-        m &= same_doc(q_pos0 + ps * torch.arange(sq), k_pos0 + ps * torch.arange(sk), list(cu))
+        m &= same_doc(q_pos0 + ps * torch.arange(sq), k_pos0 + ps * torch.arange(sk), list(cu)).to(device)
     return m
 
 
@@ -77,10 +77,10 @@ def bias(slopes, pos_q, pos_k):
 
 def chunk_bias(alibi, sq, sk):
     """The ALiBi bias of one chunk of ``sq`` rows and ``sk`` keys, ``alibi = (slopes [B, H], dist0, pstride)``: row a
-    and key c are d = pstride (a - c) + dist0 apart."""
+    and key c are d = pstride (a - c) + dist0 apart.  On the slopes' device."""
     slopes, dist0, pstride = alibi
-    return bias(slopes, pstride * torch.arange(sq, dtype=torch.int64) + int(dist0),
-                pstride * torch.arange(sk, dtype=torch.int64))
+    pos = lambda n: pstride * torch.arange(n, dtype=torch.int64, device=slopes.device)  # noqa: E731
+    return bias(slopes, pos(sq) + int(dist0), pos(sk))
 
 
 def std_slopes(H):
@@ -126,7 +126,7 @@ def chunk_forward(q, k, v, o_acc, lse, scale, mask=None, dtype=torch.float64, bi
     """``attention_oracle.chunk_forward`` under any kernel mask (``mask_of``), with a key or pair ``bias``."""
     if _delegated(mask, bias):
         return orc.chunk_forward(q, k, v, o_acc, lse, scale, mask or "none", dtype, bias)
-    p, lse_i = _softmax(_scores(q, k, scale, bias, dtype), mask_of(q.shape[1], k.shape[1], mask))
+    p, lse_i = _softmax(_scores(q, k, scale, bias, dtype), mask_of(q.shape[1], k.shape[1], mask, q.device))
     o_i = torch.einsum("bhqk,bkhd->bqhd", p, v.to(dtype))
     if o_acc is None:
         return o_i, lse_i
@@ -145,7 +145,7 @@ def chunk_backward(do, q, k, v, delta, lse, scale, mask=None, dtype=torch.float6
         return orc.chunk_backward(do, q, k, v, delta, lse, scale, mask or "none", dtype, bias)
     do, q, k, v, delta, lse = (t.to(dtype) for t in (do, q, k, v, delta, lse))
     p = torch.exp(_scores(q, k, scale, bias, dtype) - lse.unsqueeze(-1))
-    m = mask_of(q.shape[1], k.shape[1], mask)
+    m = mask_of(q.shape[1], k.shape[1], mask, q.device)
     if m is not None:
         p = p.masked_fill(~m, 0.0)
     dv = torch.einsum("bhqk,bqhd->bkhd", p, do)

@@ -1,8 +1,8 @@
 """Parity AT THE SIZES THE BENCH TIMES (BASELINE.json configs C2/C3/C4 per-GPU shapes: S_local = 32768 and
 65536, H = 32, d = 128, bf16), where a dense oracle over the whole problem does not finish:
 
-* sampled rows: for 64 random (head, row) pairs the exact O row, lse and dQ row from the fp64 oracle
-  over the FULL K/V of that head (a row of attention depends on nothing else), non-causal and causal;
+* whole heads: O, dQ, dK and dV of two heads against the fp64 oracle within the 16-bit error model, computed in
+  row blocks (``scale_model``), non-causal and causal;
 * one whole head of dK / dV against fp32 dense attention with autograd on the GPU at S = 32768;
 * the FA-style bf16 criterion of SURVEY.md 8(c): max-abs error against the fp64 oracle <= 2x the error
   of a plain bf16 PyTorch implementation of the same op (+ the hard cap of gpu_util.TOL).
@@ -18,6 +18,8 @@ pytestmark = pytest.mark.gpu
 
 from burst_attn import burst_attn_func  # noqa: E402
 from gpu_util import TOL  # noqa: E402
+from burst_attn.burst_attn_interface import _l2_block  # noqa: E402
+import scale_model as sm  # noqa: E402
 from oracle import attention_oracle as orc  # noqa: E402
 
 H, D = 32, 128
@@ -38,25 +40,16 @@ def _run(q, k, v, do, causal):
 
 @pytest.mark.parametrize("S,causal", [(32768, False), (65536, False), (65536, True)])
 def test_sampled_rows_at_bench_scale(S, causal):
+    """Whole heads (the first and a seeded one) of O, dQ, dK and dV against the row-blocked fp64 oracle within the
+    16-bit error model (``scale_model``): at this size a fixed tolerance misses a dropped key tile."""
     q, k, v, do = (_mk(S, s) for s in (101, 102, 103, 104))
-    o, dq, dk, dv = _run(q, k, v, do, causal)
-    assert not any(torch.isnan(t).any().item() for t in (o, dq, dk, dv))
-    g = torch.Generator().manual_seed(S + int(causal))
-    heads = torch.randperm(H, generator=g)[:8].tolist()
-    tol = TOL[torch.bfloat16]
-    for h in heads:
-        rows = torch.randint(0, S, (8,), generator=g).tolist()
-        if causal:
-            rows[0], rows[1] = 0, S - 1  # the extremes of the triangle
-        kh, vh = k[:, :, h:h + 1].cpu(), v[:, :, h:h + 1].cpu()
-        for r in rows:
-            n_vis = r + 1 if causal else S
-            qr, dor = q[:, r:r + 1, h:h + 1].cpu(), do[:, r:r + 1, h:h + 1].cpu()
-            # the gradient the kernel computes belongs to ITS 16-bit O (delta = rowsum(O*dO)); the oracle's
-            # dQ row uses its exact O -- the difference is inside the bf16 tolerance
-            o_ref, _, dq_ref, _, _ = orc.dense_attention_bwd(qr, kh[:, :n_vis], vh[:, :n_vis], dor)
-            torch.testing.assert_close(o[:, r:r + 1, h:h + 1].double().cpu(), o_ref, **tol)
-            torch.testing.assert_close(dq[:, r:r + 1, h:h + 1].double().cpu(), dq_ref, **tol)
+    out = _run(q, k, v, do, causal)
+    assert not any(torch.isnan(t).any().item() for t in out)
+    h = int(torch.randint(1, H, (1,), generator=torch.Generator().manual_seed(S + int(causal))))
+    blk = _l2_block()
+    sm.check_api(f"benchscale_S{S}{'_causal' if causal else ''}", out, q, k, v, do,
+                 ("causal_offset", 0) if causal else None, heads=[0, h], block=1024,
+                 seams=(blk,) if S > blk + blk // 2 else ())
 
 
 def test_one_head_dk_dv_against_fp32_dense_at_32768():
