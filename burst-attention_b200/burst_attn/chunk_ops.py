@@ -24,18 +24,25 @@ def _dims(t: torch.Tensor, seq_dim: int):
     return t.shape[0], t.shape[seq_dim], t.shape[3 - seq_dim], t.shape[3]
 
 
-def _alibi_args(alibi):
-    """(slopes fp32 [B, H], dist0, pstride) -> the C-ABI's (slopes, slopes_stride_b, dist0, pstride)."""
-    slopes, dist0, pstride = alibi
-    assert slopes.dim() == 2 and slopes.stride(1) == 1 and slopes.dtype == torch.float32
-    return slopes.data_ptr(), slopes.stride(0), int(dist0), int(pstride)
-
-
-def _doc_args(doc):
-    """(cu_seqlens int32 device, n_docs, q_pos0, k_pos0, pstride) -> the C-ABI's arguments, in that order."""
-    cu, n_docs, q_pos0, k_pos0, pstride = doc
-    assert cu.dim() == 1 and cu.dtype == torch.int32 and cu.is_contiguous()
-    return cu.data_ptr(), int(n_docs), int(q_pos0), int(k_pos0), int(pstride)
+def _mask_args(causal, causal_offset, bias, lower, alibi, doc):
+    """The chunk entry point of a call's masks and the arguments that differ between the entry points:
+    ``("_band", (key bias,), masks)``, ``("_alibi", (), masks + ALiBi)`` or ``("_doc", (), masks + documents)``, with
+    masks = (mask_mode, causal_offset, lower_offset).  The key bias goes after v in the forward, after lse in the
+    backward; the mask and variant arguments follow the scale.  A call without ALiBi or documents goes to
+    ``ba_*_chunk_band`` with or without a lower edge: with BA_MASK_LOWER clear it is ``ba_*_chunk_gqa``."""
+    masks = ((_n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE) | (0 if lower is None else _n.BA_MASK_LOWER),
+             int(causal_offset), 0 if lower is None else int(lower))
+    if doc is not None:
+        assert bias is None and alibi is None, "documents are not combined with a key bias or ALiBi"
+        cu, n_docs, q_pos0, k_pos0, pstride = doc  # cu_seqlens: int32 device boundaries
+        assert cu.dim() == 1 and cu.dtype == torch.int32 and cu.is_contiguous()
+        return "_doc", (), masks + (cu.data_ptr(), int(n_docs), int(q_pos0), int(k_pos0), int(pstride))
+    if alibi is not None:
+        assert bias is None, "ALiBi is not combined with a key bias"
+        slopes, dist0, pstride = alibi  # slopes: fp32 [B, H]
+        assert slopes.dim() == 2 and slopes.stride(1) == 1 and slopes.dtype == torch.float32
+        return "_alibi", (), masks + (slopes.data_ptr(), slopes.stride(0), int(dist0), int(pstride))
+    return "_band", (_n.rs(bias),), masks
 
 
 class NativeOps:
@@ -96,24 +103,11 @@ class NativeOps:
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         flags = (_n.BA_FWD_FIRST if first else 0) | (_n.BA_FWD_LAST if last else 0)
         e0 = self._t0(q.device)
-        args = (_n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(bias), _n.t4(o_acc, seq_dim), _n.rs(lse),
-                _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale),
-                _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
-        if doc is not None:
-            assert bias is None and alibi is None, "documents are not combined with a key bias or ALiBi"
-            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
-            rc = self.lib.ba_fwd_chunk_doc(*args[:3], *args[4:-2], mask, args[-1], 0 if lower is None else int(lower),
-                                           *_doc_args(doc), flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
-        elif alibi is not None:
-            assert bias is None, "ALiBi is not combined with a key bias"
-            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
-            rc = self.lib.ba_fwd_chunk_alibi(*args[:3], *args[4:-2], mask, args[-1], 0 if lower is None else int(lower),
-                                             *_alibi_args(alibi), flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
-        elif lower is None:
-            rc = self.lib.ba_fwd_chunk_gqa(*args, flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
-        else:
-            args = args[:-2] + (args[-2] | _n.BA_MASK_LOWER, args[-1], int(lower))
-            rc = self.lib.ba_fwd_chunk_band(*args, flags, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
+        entry, bias_arg, masks = _mask_args(causal, causal_offset, bias, lower, alibi, doc)
+        rc = getattr(self.lib, "ba_fwd_chunk" + entry)(
+            _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), *bias_arg, _n.t4(o_acc, seq_dim), _n.rs(lse),
+            _n.t4(o_out, seq_dim), B, Sq, Sk, H, H_kv, D, float(scale), *masks, flags, _n.dtype_code(q.dtype),
+            _n.stream_ptr(q.device))
         _n.check(rc, "ba_fwd_chunk")
         self._shape("fwd_chunk_kernel", Sq, Sk, H, causal)
         self._t1("fwd_chunk_kernel", e0, q.device)
@@ -136,25 +130,11 @@ class NativeOps:
         B, Sq, H, D = _dims(q, seq_dim)
         Sk, H_kv = k.shape[seq_dim], k.shape[3 - seq_dim]
         e0 = self._t0(q.device)
-        args = (_n.t4(d_o, seq_dim), _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(delta), _n.rs(lse),
-                _n.rs(bias), _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv,
-                D, float(scale), _n.BA_MASK_CAUSAL if causal else _n.BA_MASK_NONE, int(causal_offset))
-        tail = (1 if deterministic else 0, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
-        if doc is not None:
-            assert bias is None and alibi is None, "documents are not combined with a key bias or ALiBi"
-            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
-            rc = self.lib.ba_bwd_chunk_doc(*args[:6], *args[7:-2], mask, args[-1], 0 if lower is None else int(lower),
-                                           *_doc_args(doc), *tail)
-        elif alibi is not None:
-            assert bias is None, "ALiBi is not combined with a key bias"
-            mask = args[-2] | (0 if lower is None else _n.BA_MASK_LOWER)
-            rc = self.lib.ba_bwd_chunk_alibi(*args[:6], *args[7:-2], mask, args[-1], 0 if lower is None else int(lower),
-                                             *_alibi_args(alibi), *tail)
-        elif lower is None:
-            rc = self.lib.ba_bwd_chunk_gqa(*args, *tail)
-        else:
-            args = args[:-2] + (args[-2] | _n.BA_MASK_LOWER, args[-1], int(lower))
-            rc = self.lib.ba_bwd_chunk_band(*args, *tail)
+        entry, bias_arg, masks = _mask_args(causal, causal_offset, bias, lower, alibi, doc)
+        rc = getattr(self.lib, "ba_bwd_chunk" + entry)(
+            _n.t4(d_o, seq_dim), _n.t4(q, seq_dim), _n.t4(k, seq_dim), _n.t4(v, seq_dim), _n.rs(delta), _n.rs(lse),
+            *bias_arg, _n.t4(dq_acc, seq_dim), _n.t4(dk_acc, seq_dim), _n.t4(dv_acc, seq_dim), B, Sq, Sk, H, H_kv, D,
+            float(scale), *masks, 1 if deterministic else 0, _n.dtype_code(q.dtype), _n.stream_ptr(q.device))
         _n.check(rc, "ba_bwd_chunk")
         self._shape("bwd_chunk_kernel", Sq, Sk, H, causal)
         self._t1("bwd_chunk_kernel", e0, q.device)

@@ -4,23 +4,14 @@
 
 namespace ba {
 
-int launch_bwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                     const CUtensorMap& tmV, const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p,
-                     cudaStream_t stream) {
-  const bool bf16 = dtype == BA_DTYPE_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, BwdParams);
-  if (band)
-    kern = D == 64 ? (bf16 ? bwd_alibi_kernel<true, 64, true> : bwd_alibi_kernel<false, 64, true>)
-                   : (bf16 ? bwd_alibi_kernel<true, 128, true> : bwd_alibi_kernel<false, 128, true>);
-  else
-    kern = D == 64 ? (bf16 ? bwd_alibi_kernel<true, 64, false> : bwd_alibi_kernel<false, 64, false>)
-                   : (bf16 ? bwd_alibi_kernel<true, 128, false> : bwd_alibi_kernel<false, 128, false>);
-  const int smem = D == 64 ? BwdLayout<64>::kSmemBytes : BwdLayout<128>::kSmemBytes;
-  BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sk + kBwdN - 1) / kBwdN, p.H / p.G, p.B);  // one CTA per (key block, K/V head, batch)
-  kern<<<grid, kBwdThreads, smem, stream>>>(tmQ, tmK, tmV, tmDO, tmDQ, p);
-  BA_CHECK_CUDA(cudaGetLastError());
-  return BA_OK;
+BwdKernel bwd_alibi_kernel_of(bool bf16, int D, bool band) {
+  if (D == 64)
+    return {band ? (bf16 ? bwd_alibi_kernel<true, 64, true> : bwd_alibi_kernel<false, 64, true>)
+                 : (bf16 ? bwd_alibi_kernel<true, 64, false> : bwd_alibi_kernel<false, 64, false>),
+            BwdLayout<64>::kSmemBytes};
+  return {band ? (bf16 ? bwd_alibi_kernel<true, 128, true> : bwd_alibi_kernel<false, 128, true>)
+               : (bf16 ? bwd_alibi_kernel<true, 128, false> : bwd_alibi_kernel<false, 128, false>),
+          BwdLayout<128>::kSmemBytes};
 }
 
 }  // namespace ba

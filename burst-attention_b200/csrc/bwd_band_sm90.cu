@@ -4,9 +4,6 @@
 
 namespace ba {
 
-int launch_bwd_band(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                    const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream) {
-  return launch_bwd<true>(dtype, D, tmQ, tmK, tmV, tmDO, tmDQ, p, stream);
-}
+BwdKernel bwd_band_kernel_of(bool bf16, int D) { return bwd_chunk_kernel_of<true>(bf16, D); }
 
 }  // namespace ba

@@ -5,18 +5,11 @@
 
 namespace ba {
 
-int launch_bwd_doc(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                   const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream) {
-  const bool bf16 = dtype == BA_DTYPE_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, BwdParams) =
-      D == 64 ? (bf16 ? bwd_doc_kernel<true, 64> : bwd_doc_kernel<false, 64>)
-              : (bf16 ? bwd_doc_kernel<true, 128> : bwd_doc_kernel<false, 128>);
-  const int smem = D == 64 ? BwdLayout<64>::kSmemDocBytes : BwdLayout<128>::kSmemDocBytes;
-  BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sk + kBwdN - 1) / kBwdN, p.H / p.G, p.B);  // one CTA per (key block, K/V head, batch)
-  kern<<<grid, kBwdThreads, smem, stream>>>(tmQ, tmK, tmV, tmDO, tmDQ, p);
-  BA_CHECK_CUDA(cudaGetLastError());
-  return BA_OK;
+// the document kernels also stage each Q row's document keys past the other kernels' shared memory
+BwdKernel bwd_doc_kernel_of(bool bf16, int D) {
+  if (D == 64)
+    return {bf16 ? bwd_doc_kernel<true, 64> : bwd_doc_kernel<false, 64>, BwdLayout<64>::kSmemDocBytes};
+  return {bf16 ? bwd_doc_kernel<true, 128> : bwd_doc_kernel<false, 128>, BwdLayout<128>::kSmemDocBytes};
 }
 
 }  // namespace ba

@@ -667,31 +667,23 @@ bwd_doc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   bwd_chunk_body<kBF16, kD, true, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, p);
 }
 
-// the kernel of one (dtype, head dim) for this TU's kBand; bwd_sm90.cu launches kBand = false,
-// bwd_band_sm90.cu (launch_bwd_band) kBand = true
+// Each tile TU instantiates its own kernels and hands bwd_chunk_run (bwd_sm90.cu), which launches every one of them,
+// the kernel of a call's (dtype, head dim, ...) with the dynamic shared memory it needs.
+struct BwdKernel {
+  void (*fn)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, BwdParams);
+  int smem;
+};
+
+// bwd_chunk_kernel of (dtype, head dim) for this TU's kBand: bwd_sm90.cu kBand = false, bwd_band_sm90.cu true
 template <bool kBand>
-inline int launch_bwd(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                      const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream) {
-  const bool bf16 = dtype == BA_DTYPE_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, BwdParams) =
-      D == 64 ? (bf16 ? bwd_chunk_kernel<true, 64, kBand> : bwd_chunk_kernel<false, 64, kBand>)
-              : (bf16 ? bwd_chunk_kernel<true, 128, kBand> : bwd_chunk_kernel<false, 128, kBand>);
-  const int smem = D == 64 ? BwdLayout<64>::kSmemBytes : BwdLayout<128>::kSmemBytes;
-  BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sk + kBwdN - 1) / kBwdN, p.H / p.G, p.B);  // one CTA per (key block, K/V head, batch)
-  kern<<<grid, kBwdThreads, smem, stream>>>(tmQ, tmK, tmV, tmDO, tmDQ, p);
-  BA_CHECK_CUDA(cudaGetLastError());
-  return BA_OK;
+inline BwdKernel bwd_chunk_kernel_of(bool bf16, int D) {
+  if (D == 64)
+    return {bf16 ? bwd_chunk_kernel<true, 64, kBand> : bwd_chunk_kernel<false, 64, kBand>, BwdLayout<64>::kSmemBytes};
+  return {bf16 ? bwd_chunk_kernel<true, 128, kBand> : bwd_chunk_kernel<false, 128, kBand>, BwdLayout<128>::kSmemBytes};
 }
 
-int launch_bwd_band(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                    const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream);
-// bwd_alibi_sm90.cu: the ALiBi kernel of (dtype, head dim, band)
-int launch_bwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                     const CUtensorMap& tmV, const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p,
-                     cudaStream_t stream);
-// bwd_doc_sm90.cu: the document kernel of (dtype, head dim)
-int launch_bwd_doc(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                   const CUtensorMap& tmDO, const CUtensorMap& tmDQ, const BwdParams& p, cudaStream_t stream);
+BwdKernel bwd_band_kernel_of(bool bf16, int D);              // bwd_band_sm90.cu
+BwdKernel bwd_alibi_kernel_of(bool bf16, int D, bool band);  // bwd_alibi_sm90.cu
+BwdKernel bwd_doc_kernel_of(bool bf16, int D);               // bwd_doc_sm90.cu
 
 }  // namespace ba

@@ -4,9 +4,6 @@
 
 namespace ba {
 
-int launch_fwd_band(int dtype, int D, bool bias, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                    const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream) {
-  return launch_fwd<true>(dtype, D, bias, tmQ, tmK, tmV, p, stream);
-}
+FwdKernel fwd_band_kernel_of(bool bf16, int D, bool bias) { return fwd_chunk_kernel_of<true>(bf16, D, bias); }
 
 }  // namespace ba

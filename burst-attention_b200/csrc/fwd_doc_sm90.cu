@@ -5,18 +5,9 @@
 
 namespace ba {
 
-int launch_fwd_doc(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                   const FwdParams& p, cudaStream_t stream) {
-  const bool bf16 = dtype == BA_DTYPE_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams) =
-      D == 64 ? (bf16 ? fwd_doc_kernel<true, 64> : fwd_doc_kernel<false, 64>)
-              : (bf16 ? fwd_doc_kernel<true, 128> : fwd_doc_kernel<false, 128>);
-  const int smem = D == 64 ? FwdLayout<64>::kSmemBytes : FwdLayout<128>::kSmemBytes;
-  BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sq + kBlockM - 1) / kBlockM, p.H, p.B);
-  kern<<<grid, kFwdThreads, smem, stream>>>(tmQ, tmK, tmV, p);
-  BA_CHECK_CUDA(cudaGetLastError());
-  return BA_OK;
+FwdKernel fwd_doc_kernel_of(bool bf16, int D) {
+  return D == 64 ? (bf16 ? fwd_doc_kernel<true, 64> : fwd_doc_kernel<false, 64>)
+                 : (bf16 ? fwd_doc_kernel<true, 128> : fwd_doc_kernel<false, 128>);
 }
 
 }  // namespace ba

@@ -527,34 +527,22 @@ fwd_doc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   fwd_chunk_body<kBF16, kD, false, true, false, true>(tmQ, tmK, tmV, p);
 }
 
-// the kernel of one (dtype, head dim, bias) for this TU's kBand; fwd_sm90.cu launches kBand = false,
-// fwd_band_sm90.cu (launch_fwd_band) kBand = true
+// Each tile TU instantiates its own kernels and hands fwd_chunk_run (fwd_sm90.cu), which launches every one of them,
+// the kernel of a call's (dtype, head dim, ...).
+using FwdKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams);
+
+// fwd_chunk_kernel of (dtype, head dim, bias) for this TU's kBand: fwd_sm90.cu kBand = false, fwd_band_sm90.cu true
 template <bool kBand>
-inline int launch_fwd(int dtype, int D, bool bias, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                      const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream) {
-  const bool bf16 = dtype == BA_DTYPE_BF16;
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, FwdParams);
+inline FwdKernel fwd_chunk_kernel_of(bool bf16, int D, bool bias) {
   if (bias)
-    kern = D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, true, kBand> : fwd_chunk_kernel<false, 64, true, kBand>)
+    return D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, true, kBand> : fwd_chunk_kernel<false, 64, true, kBand>)
                    : (bf16 ? fwd_chunk_kernel<true, 128, true, kBand> : fwd_chunk_kernel<false, 128, true, kBand>);
-  else
-    kern = D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, false, kBand> : fwd_chunk_kernel<false, 64, false, kBand>)
-                   : (bf16 ? fwd_chunk_kernel<true, 128, false, kBand> : fwd_chunk_kernel<false, 128, false, kBand>);
-  const int smem = D == 64 ? FwdLayout<64>::kSmemBytes : FwdLayout<128>::kSmemBytes;
-  BA_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.Sq + kBlockM - 1) / kBlockM, p.H, p.B);
-  kern<<<grid, kFwdThreads, smem, stream>>>(tmQ, tmK, tmV, p);
-  BA_CHECK_CUDA(cudaGetLastError());
-  return BA_OK;
+  return D == 64 ? (bf16 ? fwd_chunk_kernel<true, 64, false, kBand> : fwd_chunk_kernel<false, 64, false, kBand>)
+                 : (bf16 ? fwd_chunk_kernel<true, 128, false, kBand> : fwd_chunk_kernel<false, 128, false, kBand>);
 }
 
-int launch_fwd_band(int dtype, int D, bool bias, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                    const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream);
-// fwd_alibi_sm90.cu: the ALiBi kernel of (dtype, head dim, band)
-int launch_fwd_alibi(int dtype, int D, bool band, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                     const CUtensorMap& tmV, const FwdParams& p, cudaStream_t stream);
-// fwd_doc_sm90.cu: the document kernel of (dtype, head dim)
-int launch_fwd_doc(int dtype, int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                   const FwdParams& p, cudaStream_t stream);
+FwdKernel fwd_band_kernel_of(bool bf16, int D, bool bias);   // fwd_band_sm90.cu
+FwdKernel fwd_alibi_kernel_of(bool bf16, int D, bool band);  // fwd_alibi_sm90.cu
+FwdKernel fwd_doc_kernel_of(bool bf16, int D);               // fwd_doc_sm90.cu
 
 }  // namespace ba

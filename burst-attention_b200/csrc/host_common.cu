@@ -76,68 +76,54 @@ int make_tensor_map(CUtensorMap* out, const ba_tensor4& t, int B, int S, int H, 
   return BA_OK;
 }
 
-int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
-                     int dtype) {
-  BA_REQUIRE(H_kv > 0 && H % H_kv == 0, "%s: H_kv=%d must be positive and divide H=%d", fn, H_kv, H);
-  BA_REQUIRE(D == 128 || D == 64, "%s: head dim %d unsupported (64 or 128)", fn, D);
-  BA_REQUIRE(B > 0 && Sq > 0 && Sk > 0 && H > 0, "%s: empty problem B=%d Sq=%d Sk=%d H=%d", fn, B, Sq, Sk, H);
-  BA_REQUIRE(dtype == BA_DTYPE_FP16 || dtype == BA_DTYPE_BF16, "%s: bad dtype %d", fn, dtype);
-  BA_REQUIRE(mask_mode == BA_MASK_NONE || mask_mode == BA_MASK_CAUSAL, "%s: bad mask mode %d", fn, mask_mode);
-  BA_REQUIRE(scale > 0.f && isfinite(scale), "%s: softmax scale must be positive and finite", fn);
-  BA_REQUIRE(H <= 65535 && B <= 65535, "%s: H and B must be <= 65535", fn);  // gridDim.y / gridDim.z
-  return BA_OK;
-}
-
-int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                    int* causal_offset, int* lower_offset, int dtype) {
-  const int mm = *mask_mode;
-  BA_REQUIRE((mm & ~(BA_MASK_CAUSAL | BA_MASK_LOWER)) == 0, "%s: bad mask mode %d", fn, mm);
-  int rc;
-  if ((rc = check_chunk_args(fn, B, Sq, Sk, H, H_kv, D, scale, mm & BA_MASK_CAUSAL, dtype))) return rc;
-  BA_REQUIRE(!(mm & BA_MASK_LOWER) || !(mm & BA_MASK_CAUSAL) || *lower_offset <= *causal_offset,
-             "%s: band lower_offset %d is above its causal_offset %d (no key would be visible)", fn, *lower_offset,
-             *causal_offset);
+int check_chunk_args(const char* fn, ChunkEntry entry, ChunkArgs* a) {
+  const int mm = a->mask_mode;
+  const int masks = entry == ChunkEntry::kPlain ? BA_MASK_CAUSAL : BA_MASK_CAUSAL | BA_MASK_LOWER;
+  // the band's entry points report a bad mask mode before anything else, the plain ones after the dtype
+  if (entry != ChunkEntry::kPlain) BA_REQUIRE((mm & ~masks) == 0, "%s: bad mask mode %d", fn, mm);
+  BA_REQUIRE(a->H_kv > 0 && a->H % a->H_kv == 0, "%s: H_kv=%d must be positive and divide H=%d", fn, a->H_kv, a->H);
+  BA_REQUIRE(a->D == 128 || a->D == 64, "%s: head dim %d unsupported (64 or 128)", fn, a->D);
+  BA_REQUIRE(a->B > 0 && a->Sq > 0 && a->Sk > 0 && a->H > 0, "%s: empty problem B=%d Sq=%d Sk=%d H=%d", fn, a->B,
+             a->Sq, a->Sk, a->H);
+  BA_REQUIRE(a->dtype == BA_DTYPE_FP16 || a->dtype == BA_DTYPE_BF16, "%s: bad dtype %d", fn, a->dtype);
+  BA_REQUIRE((mm & ~masks) == 0, "%s: bad mask mode %d", fn, mm);
+  BA_REQUIRE(a->scale > 0.f && isfinite(a->scale), "%s: softmax scale must be positive and finite", fn);
+  BA_REQUIRE(a->H <= 65535 && a->B <= 65535, "%s: H and B must be <= 65535", fn);  // gridDim.y / gridDim.z
+  BA_REQUIRE(!(mm & BA_MASK_LOWER) || !(mm & BA_MASK_CAUSAL) || a->lower_offset <= a->causal_offset,
+             "%s: band lower_offset %d is above its causal_offset %d (no key would be visible)", fn, a->lower_offset,
+             a->causal_offset);
+  if (entry == ChunkEntry::kAlibi) {
+    BA_REQUIRE(a->slopes, "%s: null ALiBi slopes", fn);
+    BA_REQUIRE((reinterpret_cast<uintptr_t>(a->slopes) & 3) == 0, "%s: ALiBi slopes must be 4-byte aligned", fn);
+    BA_REQUIRE(a->slopes_stride_b >= 0, "%s: ALiBi slopes batch stride %lld is negative", fn,
+               (long long)a->slopes_stride_b);
+    BA_REQUIRE(a->pstride >= 1, "%s: ALiBi position stride %d must be >= 1", fn, a->pstride);
+  }
+  if (entry == ChunkEntry::kDoc) {
+    BA_REQUIRE(a->cu_seqlens, "%s: null cu_seqlens", fn);
+    BA_REQUIRE((reinterpret_cast<uintptr_t>(a->cu_seqlens) & 3) == 0, "%s: cu_seqlens must be 4-byte aligned", fn);
+    BA_REQUIRE(a->n_docs >= 1, "%s: n_docs = %d must be >= 1", fn, a->n_docs);
+    BA_REQUIRE(a->pstride >= 1, "%s: position stride %d must be >= 1", fn, a->pstride);
+    BA_REQUIRE(a->q_pos0 >= 0 && a->k_pos0 >= 0, "%s: positions q_pos0 = %lld, k_pos0 = %lld must be >= 0", fn,
+               (long long)a->q_pos0, (long long)a->k_pos0);
+    // cu_seqlens is int32, so every position is; the kernels count positions in 32 bits
+    BA_REQUIRE(a->q_pos0 + (int64_t)a->pstride * (a->Sq - 1) <= INT32_MAX &&
+                   a->k_pos0 + (int64_t)a->pstride * (a->Sk - 1) <= INT32_MAX,
+               "%s: the positions of the rows or keys exceed int32", fn);
+  }
   // The kernels add the causal offset to row and key indices in 32-bit arithmetic.  An offset >= Sk - 1 shows every
   // key to every row and one <= -Sq shows none, so clamping it into [-Sq, Sk] changes no mask and keeps those sums in
   // range.  A lower edge at or below the causal one stays there: both clamps below are monotone, and a clamped lower
   // edge is at most Sk.
-  *causal_offset = *causal_offset > Sk ? Sk : *causal_offset < -Sq ? -Sq : *causal_offset;
-  if (!(mm & BA_MASK_LOWER)) return BA_OK;
+  a->causal_offset = a->causal_offset > a->Sk ? a->Sk : a->causal_offset < -a->Sq ? -a->Sq : a->causal_offset;
   // a lower edge at or below key 0 for every row (lower_offset <= 1 - Sq) masks nothing: run the kernel without one;
   // one at or above Sk masks every key of every row, as lower_offset = Sk does (and row + Sk cannot overflow)
-  if (*lower_offset <= 1 - Sq) *mask_mode = mm & ~BA_MASK_LOWER;
-  else if (*lower_offset > Sk) *lower_offset = Sk;
-  return BA_OK;
-}
-
-int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                     int* causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
-                     int dtype) {
-  int rc;
-  if ((rc = check_band_args(fn, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset, lower_offset, dtype)))
-    return rc;
-  BA_REQUIRE(slopes, "%s: null ALiBi slopes", fn);
-  BA_REQUIRE((reinterpret_cast<uintptr_t>(slopes) & 3) == 0, "%s: ALiBi slopes must be 4-byte aligned", fn);
-  BA_REQUIRE(slopes_stride_b >= 0, "%s: ALiBi slopes batch stride %lld is negative", fn, (long long)slopes_stride_b);
-  BA_REQUIRE(pstride >= 1, "%s: ALiBi position stride %d must be >= 1", fn, pstride);
-  return BA_OK;
-}
-
-int check_doc_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                   int* causal_offset, int* lower_offset, const int* cu_seqlens, int n_docs, int64_t q_pos0,
-                   int64_t k_pos0, int pstride, int dtype) {
-  int rc;
-  if ((rc = check_band_args(fn, B, Sq, Sk, H, H_kv, D, scale, mask_mode, causal_offset, lower_offset, dtype)))
-    return rc;
-  BA_REQUIRE(cu_seqlens, "%s: null cu_seqlens", fn);
-  BA_REQUIRE((reinterpret_cast<uintptr_t>(cu_seqlens) & 3) == 0, "%s: cu_seqlens must be 4-byte aligned", fn);
-  BA_REQUIRE(n_docs >= 1, "%s: n_docs = %d must be >= 1", fn, n_docs);
-  BA_REQUIRE(pstride >= 1, "%s: position stride %d must be >= 1", fn, pstride);
-  BA_REQUIRE(q_pos0 >= 0 && k_pos0 >= 0, "%s: positions q_pos0 = %lld, k_pos0 = %lld must be >= 0", fn,
-             (long long)q_pos0, (long long)k_pos0);
-  // cu_seqlens is int32, so every position is; the kernels count positions in 32 bits
-  BA_REQUIRE(q_pos0 + (int64_t)pstride * (Sq - 1) <= INT32_MAX && k_pos0 + (int64_t)pstride * (Sk - 1) <= INT32_MAX,
-             "%s: the positions of the rows or keys exceed int32", fn);
+  if (mm & BA_MASK_LOWER) {
+    if (a->lower_offset <= 1 - a->Sq) a->mask_mode = mm & ~BA_MASK_LOWER;
+    else if (a->lower_offset > a->Sk) a->lower_offset = a->Sk;
+  }
+  // documents run on the band path: without a lower edge, one that masks nothing (row + 1 - Sq <= 0 <= key)
+  if (entry == ChunkEntry::kDoc && !(a->mask_mode & BA_MASK_LOWER)) a->lower_offset = 1 - a->Sq;
   return BA_OK;
 }
 

@@ -48,28 +48,37 @@ inline bool aligned16(const ba_tensor4& t, int esize) {
          t.stride_h % q == 0;
 }
 
-// Preconditions shared by the forward and backward chunk entry points; `fn` names the entry point in the error
-// message.  Returns BA_OK or BA_ERR_INVALID.
-int check_chunk_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int mask_mode,
-                     int dtype);
+// The arguments of one forward or backward chunk call besides its operands: the problem, the mask, and the optional
+// key bias, ALiBi and documents.  Fields up to lower_offset are in the entry points' parameter order.
+struct ChunkArgs {
+  int B, Sq, Sk, H, H_kv, D;
+  float scale;
+  int mask_mode, causal_offset, lower_offset;
+  int dtype;
+  ba_rowstat key_bias = {nullptr, 0, 0};  // null: no key bias
+  const float* slopes = nullptr;          // ALiBi; null: none
+  int64_t slopes_stride_b = 0, dist0 = 0;
+  const int* cu_seqlens = nullptr;        // documents; null: none
+  int n_docs = 0;
+  int64_t q_pos0 = 0, k_pos0 = 0;
+  int pstride = 1;                        // ALiBi and documents
+};
 
-// The same for the band entry points, whose mask_mode is a set of BA_MASK_CAUSAL and BA_MASK_LOWER bits; every
-// forward and backward entry point ends up here.  On success it normalises the masks without changing which keys
-// are visible: *causal_offset is clamped into [-Sq, Sk] (beyond either end it shows every key or none, and the
-// kernels' 32-bit index sums with it stay in range), a lower edge that masks nothing is dropped from *mask_mode, and
-// *lower_offset is clamped to Sk -- still at or below the clamped causal offset.
-int check_band_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                    int* causal_offset, int* lower_offset, int dtype);
+// Which family of entry points a chunk call came through, and so which of its arguments are checked.
+//   kPlain  ba_*_chunk, _bias, _gqa: mask_mode is BA_MASK_NONE or BA_MASK_CAUSAL
+//   kBand   ba_*_chunk_band: mask_mode is a set of BA_MASK_CAUSAL and BA_MASK_LOWER bits
+//   kAlibi  ba_*_chunk_alibi: the band's masks, plus the slopes (non-null, 4-byte aligned, batch stride >= 0) and
+//           pstride >= 1
+//   kDoc    ba_*_chunk_doc: the band's masks, plus the boundaries (non-null, 4-byte aligned, n_docs >= 1),
+//           pstride >= 1 and positions q_pos0, k_pos0 >= 0 whose last row and key still fit in int32
+enum class ChunkEntry { kPlain, kBand, kAlibi, kDoc };
 
-// The same for the ALiBi entry points: check_band_args, plus the slopes (non-null, batch stride >= 0) and pstride >= 1.
-int check_alibi_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                     int* causal_offset, int* lower_offset, const float* slopes, int64_t slopes_stride_b, int pstride,
-                     int dtype);
-
-// The same for the document entry points: check_band_args, plus the boundaries (non-null, 4-byte aligned,
-// n_docs >= 1), pstride >= 1 and positions q_pos0, k_pos0 >= 0 whose last row and key still fit in int32.
-int check_doc_args(const char* fn, int B, int Sq, int Sk, int H, int H_kv, int D, float scale, int* mask_mode,
-                   int* causal_offset, int* lower_offset, const int* cu_seqlens, int n_docs, int64_t q_pos0,
-                   int64_t k_pos0, int pstride, int dtype);
+// The preconditions of every forward and backward chunk entry point; `fn` names the entry point in the error message.
+// Returns BA_OK or BA_ERR_INVALID.  On success it normalises the masks without changing which keys are visible:
+// causal_offset is clamped into [-Sq, Sk] (beyond either end it shows every key or none, and the kernels' 32-bit index
+// sums with it stay in range), a lower edge that masks nothing is dropped from mask_mode, and lower_offset is clamped
+// to Sk -- still at or below the clamped causal offset.  Documents always run with a lower edge: without
+// BA_MASK_LOWER it is 1 - Sq, which masks nothing.
+int check_chunk_args(const char* fn, ChunkEntry entry, ChunkArgs* a);
 
 }  // namespace ba

@@ -19,7 +19,7 @@ BWD_M, BWD_N = 64, 128  # backward: rows per Q block, keys per CTA
 
 
 def normalise(Sq, Sk, causal, causal_off, lower):
-    """check_band_args + the doc entries' lower edge: (causal_off, lo) as the kernels get them."""
+    """check_chunk_args for the doc entries (csrc/host_common.cu): (causal_off, lo) as the kernels get them."""
     off = max(-Sq, min(Sk, causal_off)) if causal else causal_off
     if lower is None or lower <= 1 - Sq:
         lo = 1 - Sq  # masks nothing: row + 1 - Sq <= 0 <= key

@@ -168,7 +168,7 @@ def bwd_q_range(k0, sq, sk, lo, hi):
 
 
 def host_lower(sq, sk, lo, mutant=None):
-    """The lower edge the kernels get from ``check_band_args`` (None: dropped, the kernel without one runs)."""
+    """The lower edge the kernels get from ``check_chunk_args`` (csrc/host_common.cu) (None: dropped, the kernel without one runs)."""
     if lo is None:
         return None
     if lo <= (2 if mutant == "band_drop_at_2_minus_sq" else 1) - sq:
