@@ -14,8 +14,10 @@ the copies can ride under the kernels instead of bracketing the call:
 Exposed at S = 262144 (H = 32, d = 128): Q + the first K/V block up (2.6 GB) and the last dQ / dK / dV blocks down
 (0.8 GB) out of 17 GB each way.  Device memory: the 16-bit Q, K, V, O stay resident between forward and backward.
 
-Contract (the same as ``tensor.to("cpu", non_blocking=True)``): the returned host tensors are complete after
-``torch.cuda.synchronize()``; the compute stream itself is made to wait for every copy at the end of the backward.
+Contract: the forward's O is returned like ``tensor.to("cpu", non_blocking=True)``: it rides down under the backward
+and is complete after ``torch.cuda.synchronize()``.  The backward's dQ / dK / dV are complete when it returns: the host
+waits for their last blocks to land, because autograd hands them to CPU consumers at once (``q.grad += dq`` when
+gradients accumulate, tensor hooks, CPU ops upstream of q); the compute stream is made to wait for every copy as well.
 Only W = 1 (no ring); with W > 1 pass device tensors.
 """
 from __future__ import annotations
@@ -151,5 +153,10 @@ def backward(d_o, saved, scale, seq_dim, band, blk, deterministic):
         ship(dq_acc, dq16, dq_h, r0, rn)
     for t in (dq16, dk16, dv16):
         t.record_stream(down)
+    # autograd hands the gradients to CPU consumers as soon as this returns (AccumulateGrad's q.grad += dq, tensor
+    # hooks, CPU ops upstream of q): the host waits for the last blocks to land
+    landed = torch.cuda.Event()
+    landed.record(down)
+    landed.synchronize()
     cur.wait_stream(down)  # stream order: whatever follows on the compute stream sees complete host gradients
     return dq_h, dk_h, dv_h
